@@ -253,7 +253,8 @@ int tgb200_unpack_tiles(tgb_ctx *ctx, const tgb_tile *tiles, uint32_t n_tiles, c
  * Host only.                                                                                                          */
 int tgb200_shard_tiles(const tgb_tile *tiles, uint32_t n_tiles, uint32_t *order);
 
-/* Batch of closest-hit queries through the same traversal kernel the renderer uses.                 */
+/* Batch of closest-hit queries through the same traversal kernel the renderer uses.  As in a render, a ray that misses the
+ * BVH's top-level cut before its analytic hit skips the traversal; environment TGB_HOOK_CUT=0 traverses every ray.        */
 int tgb200_trace_closest(tgb_ctx *ctx, const tgb_ray *rays, tgb_hit *hits, uint32_t n);
 
 int  tgb200_get_stats(tgb_ctx *ctx, tgb_stats *out);
@@ -297,6 +298,15 @@ int  tgb200_bsdf_sample_probe(tgb_ctx *ctx, uint32_t seed, uint32_t n, const int
 int  tgb200_light_probe(tgb_ctx *ctx, int prim, uint32_t seed, uint32_t n, uint32_t sample, const float *p, float *out);
 int  tgb200_choose_light_probe(tgb_ctx *ctx, uint32_t seed, uint32_t n, const uint32_t *pixel_id, uint32_t sample, const float *p,
                                float *out);
+/* tgb200_shadow_probe: TraceBase::attenuatedEmission of n queries through the renderer's own shadow kernels.  Query i = 8 floats
+ * (point p.xyz, direction d.xyz, epsilon, arg) + 2 ints light_mis = (light primitive, mis).  A NEE query (mis = 0, arg = the
+ * expected distance) is set up as the shading kernel sets up lightSample's with f = 1, pdfL = 1, pdfB = 0; a MIS query (mis = 1,
+ * arg = the BSDF pdf) as bsdfSample's with weight = 1.  Then the analytic / cut pass and the BVH pass run as in a render, in
+ * chunks of the context's capacity.  out = 8 floats per query: light hit (mesh lights: 1), t of the light (mesh lights: 0), vis,
+ * the finished lightF / bsdfF rgb (emission, or emission x the power heuristic for MIS; counts only when vis = 1), queued
+ * (0: no query, 1: settled by the analytic / cut pass, 2: reached the BVH pass), traced as a blocker test.  A failed probe
+ * still restores them unless the device itself faulted.  The context's control block and ray counters are left as they were. */
+int  tgb200_shadow_probe(tgb_ctx *ctx, uint32_t n, const float *query, const int *light_mis, float *out);
 /* tgb200_abort cancels the render in progress (it returns TGB_ERR_ABORTED) or, if none is running, the next one -- so an
  * abort that lands between an asynchronous start and the worker reaching the render call is not lost.  A caller that
  * starts renders asynchronously calls tgb200_clear_abort before spawning the worker (the adapter's startRender does).   */

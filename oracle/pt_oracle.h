@@ -54,6 +54,7 @@ int      oracle_bsdf_sample_lobes(oracle_scene *s, uint32_t seed, uint32_t suppl
 int      oracle_light_probe_mode(oracle_scene *s, int prim, uint32_t seed, uint32_t supplemental_mode, int n, uint32_t sample,
                                  const float *p, float *out);
 int      oracle_choose_light(oracle_scene *s, uint32_t seed, int n, const uint32_t *pixel_id, uint32_t sample, const float *p, float *out);
+int      oracle_shadow_probe(oracle_scene *s, int n, const float *query, const int *light_mis, float *out);
 int      oracle_hair_eval(float roughness, float scale_angle_deg, const float *sigma_a, const float *wi_wo, int n, float *out);
 int      oracle_hair_tables(float roughness, float scale_angle_deg, const float *sigma_a, float *tables, float *sums, float *v);
 

@@ -55,6 +55,8 @@ def lib():
         L.oracle_light_probe_mode.argtypes = [vp, C.c_int, u32, u32, C.c_int, u32, vp, vp]
         L.oracle_choose_light.restype = C.c_int
         L.oracle_choose_light.argtypes = [vp, u32, C.c_int, vp, u32, vp, vp]
+        L.oracle_shadow_probe.restype = C.c_int
+        L.oracle_shadow_probe.argtypes = [vp, C.c_int, vp, vp, vp]
         _LIB = L
     return _LIB
 

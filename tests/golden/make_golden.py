@@ -651,6 +651,8 @@ def make_scenes(only=None):
     # the two emitters of the shipped hair scene: infinite_sphere_cap (sampled sun) + skydome (unsampled sky); min_bounces 1 as shipped
     scenes["hair_sky"] = synth.hair_scene(os.path.join(HERE, "hair_sky"), "scene", n_curves=300, res=res, spp=spp, shipped_lights=True, min_bounces=1)
     dump_sky_image(scenes["hair_sky"], os.path.join(HERE, "hair_sky", "scene_sky.pfm"))
+    # lights flush with a blocker (a shadow query's blocker at exactly the light's distance): which tie rule the reference follows
+    scenes["flush_lights"] = synth.flush_lights(os.path.join(HERE, "flush_lights"), "scene", res=res, spp=spp)
     # adaptive sampling (PathTraceIntegrator::generateWork): three 16-spp steps, the 2nd and 3rd distributed by the blocks' error
     ad = synth.cornell_box(res=res, spp=48)
     ad["renderer"].update(adaptive_sampling=True, spp_step=16)

@@ -94,6 +94,9 @@ def test_probe_hooks_refuse_a_missing_context():
                                       buf.ctypes.data, pix.ctypes.data) == abi.TGB_ERR_INVALID
     assert L.tgb200_light_probe(None, 0, 0, 1, 0, buf.ctypes.data, buf.ctypes.data) == abi.TGB_ERR_INVALID
     assert L.tgb200_choose_light_probe(None, 0, 1, pix.ctypes.data, 0, buf.ctypes.data, buf.ctypes.data) == abi.TGB_ERR_INVALID
+    lm = np.zeros(2, np.int32)
+    assert L.tgb200_shadow_probe(None, 1, buf.ctypes.data, lm.ctypes.data, buf.ctypes.data) == abi.TGB_ERR_INVALID
+    assert L.tgb200_shadow_probe(None, 0, None, None, None) == abi.TGB_ERR_INVALID
 
 
 def test_product_never_imports_the_oracle():

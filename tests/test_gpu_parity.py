@@ -169,21 +169,50 @@ def test_small_capacity_chunks_pixels_and_samples(scratch):
     assert np.array_equal(a, b)
 
 
-def test_trace_closest_hit_ids(scratch):
-    fs = scene.load_scene(synth.material_room(scratch, name="hits", res=(32, 32), spp=1, subdiv=4))
-    rng = np.random.RandomState(7)
-    n = 200000
+def _hit_rays(rng, n, ref_trace):
+    """Random rays plus the strata where a traversal goes wrong: axis-parallel directions whose other components are exactly +-0 or
+    1e-31 (below the 1e-30 clamp of the inverse direction), and finite tmax just before and just after a known hit.  Every origin
+    lies inside the room (x, z in [-0.9, 0.9], y in [0.05, 1.9]): the BVH's padding of its boxes assumes origins within the
+    scene's and the camera's extent (tgb200_api.cu, the quantised node boxes)."""
     o = rng.uniform(-0.9, 0.9, (n, 3)).astype(np.float32); o[:, 1] = rng.uniform(0.05, 1.9, n)
     d = rng.normal(size=(n, 3)).astype(np.float32); d /= np.linalg.norm(d, axis=1, keepdims=True)
+    k = n//8
+    ax = np.zeros((k, 3), np.float32); a = rng.randint(0, 3, k); ax[np.arange(k), a] = rng.choice([-1.0, 1.0], k)
+    z = rng.randint(0, 3, (k, 3))
+    tiny = np.where(z == 1, np.float32(-0.0), np.where(z == 2, np.float32(1e-31)*rng.choice([-1, 1], (k, 3)), np.float32(0.0)))
+    d[:k] = np.where(ax == 0, tiny, ax).astype(np.float32)
     rays = np.concatenate([o, d, np.full((n, 1), 5e-4, np.float32), np.full((n, 1), np.inf, np.float32)], axis=1)
-    orc = pyoracle.Oracle(fs); ref = orc.trace(rays); orc.close()
-    ctx = lib.Context(fs); got = ctx.trace_closest(rays); ctx.close()
+    # finite tmax: one ulp before / at / one ulp after the oracle's closest hit of the same ray
+    t = ref_trace(rays)["t"]
+    m = np.isfinite(t); idx = np.flatnonzero(m)[: n//4]
+    fin = rays[idx].copy()
+    sel = rng.randint(0, 3, len(idx))
+    fin[:, 7] = np.where(sel == 0, np.nextafter(t[idx], np.float32(0)), np.where(sel == 1, t[idx], np.nextafter(t[idx], np.float32(np.inf))))
+    return np.concatenate([rays, fin]).astype(np.float32)
+
+
+def test_trace_closest_hit_ids(scratch, monkeypatch):
+    """Hit ids against the oracle with the BVH's top-level cut applied as in a render (the default) and with TGB_HOOK_CUT=0: the
+    two must be identical."""
+    fs = scene.load_scene(synth.material_room(scratch, name="hits", res=(32, 32), spp=1, subdiv=4))
+    orc = pyoracle.Oracle(fs)
+    rays = _hit_rays(np.random.RandomState(7), 200000, orc.trace)
+    ref = orc.trace(rays); orc.close()
+    ctx = lib.Context(fs)
+    got = ctx.trace_closest(rays)
+    monkeypatch.setenv("TGB_HOOK_CUT", "0")
+    nocut = ctx.trace_closest(rays)
+    monkeypatch.delenv("TGB_HOOK_CUT")
+    ctx.close()
+    assert got.tobytes() == nocut.tobytes(), "the top-level cut changed a hit"
     same = (ref["primitive"] == got["primitive"]) & (ref["prim_id"] == got["prim_id"])
     # ties: equal t within 4 ulp
     with np.errstate(invalid="ignore"):      # inf - inf for rays that miss on both sides
         tie = np.abs(ref["t"] - got["t"]) <= 4*np.spacing(np.abs(ref["t"]).astype(np.float32))
     bad = ~same & ~tie
-    print("hit ids equal %.6f, ties %d, bad %d" % (same.mean(), int((~same & tie).sum()), int(bad.sum())))
+    fin = np.isfinite(rays[:, 7])
+    print("hit ids equal %.6f, ties %d, bad %d; finite tmax: %d rays, %d hits" % (same.mean(), int((~same & tie).sum()), int(bad.sum()),
+                                                                                int(fin.sum()), int((got["primitive"][fin] >= 0).sum())))
     assert bad.sum() == 0
     assert np.array_equal(ref["t"][same], got["t"][same])
     assert np.array_equal(ref["backside"][same], got["backside"][same])

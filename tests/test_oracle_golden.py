@@ -73,6 +73,25 @@ def test_curve_scenes_close(name, mode, ref):
     assert abs(float(img.mean()) - float(want.mean())) <= 5e-3*float(want.mean())
 
 
+@pytest.mark.parametrize("mode,ref", [(0, "ref_pathseed.pfm"), (1, "ref_stock.pfm")])
+def test_flush_lights_ties_follow_embree_order(mode, ref):
+    """Lights flush with a blocker (synth.flush_lights): a shadow ray's closest hit ties between the light and the quad or mesh it
+    lies in.  The reference takes whichever of the two Embree's BVH visits last (quads: Quad::intersect accepts t == farT) or
+    first (triangles); the oracle takes the later-listed quad and its own BVH's first triangle.  Embree's order is not list
+    order: reversing the oracle's quad order raises this scene to 84 % exact but costs cornell its bit-exactness.  Measured:
+    74.2 / 74.1 % of pixels exact, 74.4 / 74.2 % close, mean 5.7 % below the reference's (pathseed / stock); the other pixels and
+    every other fixture are unaffected.  Bars: >= 72 % close, mean within 7 %."""
+    img = _render("flush_lights", mode)
+    want = scene.load_pfm(os.path.join(G, "flush_lights", ref))
+    d = np.abs(img - want).max(axis=2)
+    exact = float((d == 0).mean())
+    close = float((d <= 1e-5*(1.0 + np.abs(want).max(axis=2))).mean())
+    rel = abs(float(img.mean()) - float(want.mean()))/float(want.mean())
+    print("flush_lights", mode, "exact %.4f close %.4f mean off %.4f" % (exact, close, rel))
+    assert close >= 0.72
+    assert rel <= 0.07
+
+
 def test_pathseed_and_stock_references_differ():
     a = scene.load_pfm(os.path.join(G, "cornell", "ref_pathseed.pfm"))
     b = scene.load_pfm(os.path.join(G, "cornell", "ref_stock.pfm"))

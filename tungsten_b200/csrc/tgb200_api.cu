@@ -66,7 +66,7 @@ struct tgb_ctx {
     bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
     bool has_curves = false;        // selects the kernel instantiations with the curve-segment test and per-hit epsilon
-    int n_bsdfs = 0; std::vector<uint32_t> prim_types;      // host copies for the test hooks' argument checks
+    int n_bsdfs = 0; std::vector<uint32_t> prim_types; std::vector<int> light_ids;   // host copies for the test hooks' argument checks
     uint32_t *bin_keys = nullptr, *bin_hist = nullptr;
     size_t res_capacity = 0;
     Ctl *ctl = nullptr;             // device-resident loop control block
@@ -683,6 +683,7 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
     c->n_bsdfs = int(bsdfs.size());
     c->prim_types.resize(prims.size());
     for (size_t i = 0; i < prims.size(); ++i) c->prim_types[i] = prims[i].type;
+    c->light_ids = lights;
     std::vector<uint32_t> slots(d->bsdf_slots, d->bsdf_slots + d->n_bsdf_slots);
     if ((rc = dev_upload(c, &sc.slots, slots))) return rc;
     if ((rc = dev_upload(c, &sc.tex, dtex))) return rc;
@@ -1317,26 +1318,38 @@ int tgb200_framebuffer_device_ptr(tgb_ctx *c, void **rgb_mean_dev, uint64_t *n_b
 }
 
 // Closest hits of n device rays through the analytic pass and the renderer's traversal kernels (into device Hit records)
+// As in a render, rays that miss the BVH's top-level cut before their analytic hit skip the traversal (TGB_HOOK_CUT=0: every ray
+// is traversed).
 static cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t n) {
-    k_hook_analytic<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, n);
-    c->stats.kernel_launches++;
-    if (c->sc.n_nodes) {
+    const char *cut_env = getenv("TGB_HOOK_CUT");
+    const int cut = (cut_env && cut_env[0] == '0') ? 0 : 1;
+    uint32_t *list = nullptr;                                   // [count | indices of the rays to traverse]
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&list), (size_t(n) + 1)*sizeof(uint32_t), c->stream);
+    if (e != cudaSuccess) return e;
+    e = cudaMemsetAsync(list, 0, sizeof(uint32_t), c->stream);
+    if (e == cudaSuccess) {
+        k_hook_analytic<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, n, cut, list + 1, list);
+        c->stats.kernel_launches++;
+    }
+    if (e == cudaSuccess && c->sc.n_nodes) {
         // the renderer's own persistent kernel body: treelet staged in shared memory, lane refill (TGB_HOOK_SIMPLE=1: one ray
         // per thread, nodes from global memory only)
         const char *simple = getenv("TGB_HOOK_SIMPLE");
         if (simple && simple[0] == '1') {
-            if (c->has_curves) k_hook_bvh<true><<<blocks(n, kTraceBlock), kTraceBlock, kStackSmemBytes, c->stream>>>(c->sc, dr, dx, n);
-            else k_hook_bvh<false><<<blocks(n, kTraceBlock), kTraceBlock, kStackSmemBytes, c->stream>>>(c->sc, dr, dx, n);
+            if (c->has_curves) k_hook_bvh<true><<<blocks(n, kTraceBlock), kTraceBlock, kStackSmemBytes, c->stream>>>(c->sc, dr, dx, list + 1, list, n);
+            else k_hook_bvh<false><<<blocks(n, kTraceBlock), kTraceBlock, kStackSmemBytes, c->stream>>>(c->sc, dr, dx, list + 1, list, n);
         } else {
-            cudaError_t e = cudaMemsetAsync(&c->ctl->cursor_trace, 0, sizeof(uint32_t), c->stream);
-            if (e != cudaSuccess) return e;
+            e = cudaMemsetAsync(&c->ctl->cursor_trace, 0, sizeof(uint32_t), c->stream);
             uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
-            if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, c->trace_smem, c->stream>>>(c->sc, dr, dx, n, &c->ctl->cursor_trace);
-            else k_hook_persist<false><<<grid, kTraceBlock, c->trace_smem, c->stream>>>(c->sc, dr, dx, n, &c->ctl->cursor_trace);
+            if (e == cudaSuccess) {
+                if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, c->trace_smem, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
+                else k_hook_persist<false><<<grid, kTraceBlock, c->trace_smem, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
+            }
         }
         c->stats.kernel_launches++;
     }
-    return cudaSuccess;
+    const cudaError_t ef = cudaFreeAsync(list, c->stream);
+    return e != cudaSuccess ? e : ef;
 }
 
 int tgb200_trace_closest(tgb_ctx *c, const tgb_ray *rays, tgb_hit *hits, uint32_t n) {
@@ -1867,6 +1880,54 @@ int tgb200_choose_light_probe(tgb_ctx *c, uint32_t seed, uint32_t n, const uint3
         e = b.download(out, dout, 2*size_t(n));
     }
     return b.finish(e, "choose_light_probe");
+}
+
+int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *light_mis, float *out) {
+    if (!c || (n && (!query || !light_mis || !out))) return TGB_ERR_INVALID;
+    for (uint32_t i = 0; i < n; ++i)
+        if (std::find(c->light_ids.begin(), c->light_ids.end(), light_mis[2*size_t(i)]) == c->light_ids.end())
+            return fail(c, TGB_ERR_INVALID, "query %u: primitive %d is not a samplable light", i, light_mis[2*size_t(i)]);
+    if (n == 0) return TGB_OK;
+    CU(cudaSetDevice(c->device));
+    ProbeBufs b(c);
+    float *dq = nullptr, *dout = nullptr; int *dl = nullptr; Ctl *ctl_saved = nullptr; Counters *ctr_saved = nullptr;
+    cudaError_t e = b.upload(&dq, query, 8*size_t(n));
+    if (e == cudaSuccess) e = b.upload(&dl, light_mis, 2*size_t(n));
+    if (e == cudaSuccess) e = b.alloc(&dout, 8*size_t(n));
+    if (e == cudaSuccess) e = b.alloc(&ctl_saved, 1);
+    if (e == cudaSuccess) e = b.alloc(&ctr_saved, 1);
+    // the probe's queries must not show in the context's control block or in the next render's statistics
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, c->ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
+    const bool saved = e == cudaSuccess;
+    const DScene &sc = c->sc; const bool curves = c->has_curves; cudaStream_t st = c->stream;
+    // one scratch slot per query: chunks of the context's capacity
+    for (uint32_t off = 0; off < n && e == cudaSuccess; off += c->capacity) {
+        const uint32_t m = std::min(c->capacity, n - off);
+        // shadow_count, shadow_count2, cursor_trace, cursor_shadow
+        e = cudaMemsetAsync(&c->ctl->shadow_count, 0, 4*sizeof(uint32_t), st);
+        if (e != cudaSuccess) break;
+        k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, c->sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
+                                                            c->squeue, c->ctl, m);
+        if (curves) k_shadow_prep<true><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->ctr);
+        else k_shadow_prep<false><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->ctr);
+        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(c->squeue2, c->ctl, dout + 8*size_t(off));
+        if (sc.n_nodes) {
+            const uint32_t grid = std::min(blocks(m, kTraceBlock), c->persist_blocks);
+            if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
+            else k_shadow_bvh<false><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
+        }
+        k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(c->sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
+        e = cudaGetLastError();
+    }
+    // restored also when a launch failed (the copies are queued after whatever was queued)
+    if (saved) {
+        const cudaError_t r1 = cudaMemcpyAsync(c->ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, st);
+        const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
+    }
+    if (e == cudaSuccess) e = b.download(out, dout, 8*size_t(n));
+    return b.finish(e, "shadow_probe");
 }
 
 int tgb200_clear_abort(tgb_ctx *c) {

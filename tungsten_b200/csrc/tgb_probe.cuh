@@ -1,6 +1,7 @@
-// Kernels of the test hooks (tgb200_bsdf_probe, tgb200_bsdf_sample_probe, tgb200_light_probe, tgb200_choose_light_probe): one
-// thread per input, each calling the device functions k_shade calls (bsdf_eval / bsdf_pdf / bsdf_sample with k_shade's template
-// arguments, light_sample_direct + light_hit_direct / mesh_direct_pdf, choose_light).  Nothing here restates their arithmetic.
+// Kernels of the test hooks (tgb200_bsdf_probe, tgb200_bsdf_sample_probe, tgb200_light_probe, tgb200_choose_light_probe,
+// tgb200_shadow_probe): one thread per input, each calling the device functions k_shade calls (bsdf_eval / bsdf_pdf / bsdf_sample
+// with k_shade's template arguments, light_sample_direct + light_hit_direct / mesh_direct_pdf, choose_light, light_query).
+// Nothing here restates their arithmetic.
 #pragma once
 #include "tgb_wavefront.cuh"
 
@@ -92,6 +93,50 @@ __global__ void __launch_bounds__(128) k_probe_light_mesh(DScene sc, int li, con
     const V3 em = eval_direct(sc, ls);
     float *o = out + 12*size_t(i);
     o[6] = 1.0f; o[7] = h.t; o[8] = mesh_direct_pdf(sc.prims[li], pt, d, ls); o[9] = em.x; o[10] = em.y; o[11] = em.z;
+}
+
+// tgb200_shadow_probe, before k_shadow_prep / k_shadow_bvh: query i gets scratch slot i and the records k_shade writes for it
+// (light_query with f = 1, pdfL = 1, pdfB = 0 for NEE, weight = 1 and the given BSDF pdf for MIS), and is queued when k_shade
+// would queue it.  out = 8 floats per query: light hit, t of the light, vis, finished value.rgb (filled in by k_probe_shadow_read),
+// queued (1; 2 once k_probe_shadow_traversed saw it reach the BVH pass), any.  query = 8 floats: p.xyz, d.xyz, epsilon, arg (NEE: expected distance, MIS: BSDF pdf); light_mis = 2 ints.
+__global__ void __launch_bounds__(128) k_probe_shadow_setup(DScene sc, Scratch sr, const float *query, const int *light_mis, float *out,
+                                                            uint32_t *squeue, Ctl *ctl, uint32_t n) {
+    const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float *q = query + 8*size_t(i);
+    const V3 p = v3(q[0], q[1], q[2]), d = v3(q[3], q[4], q[5]);
+    const float eps = q[6], arg = q[7];
+    const int li = light_mis[2*size_t(i)]; const bool mis = light_mis[2*size_t(i) + 1] != 0;
+    const DPrim &l = sc.prims[li];
+    float4 nx = make_float4(0.0f, 0.0f, 0.0f, 0.0f), mx = nx; float t = INFINITY; bool any = false;
+    const bool queued = light_query(sc, l, p, d, eps, mis, v3s(1.0f), mis ? arg : 1.0f, 0.0f, arg, mis ? mx : nx, t, any);
+    sr.P[i] = make_float4(p.x, p.y, p.z, eps);
+    if (mis) sr.M0[i] = make_float4(d.x, d.y, d.z, t); else sr.N0[i] = make_float4(d.x, d.y, d.z, t);
+    sr.N1[i] = nx; sr.M1[i] = mx;
+    sr.D1[i] = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(li));
+    *reinterpret_cast<uint2 *>(sr.vis + 2*size_t(i)) = make_uint2(0u, 0u);
+    if (queued) squeue[atomicAdd(&ctl->shadow_count, 1u)] = (i << 2) | (mis ? 1u : 0u) | (any ? 2u : 0u);
+    float *o = out + 8*size_t(i);
+    o[0] = 1.0f; o[1] = 0.0f;                            // mesh lights: the hit is the traversal's (vis)
+    if (l.type != TGB_PRIM_MESH) {                       // the light's own hit, also when light_query found it emits nothing
+        V3 em; float directPdf;
+        o[0] = light_hit_direct(sc, l, p, d, eps, mis ? -1.0f : arg, em, o[1], directPdf) ? 1.0f : 0.0f;
+    }
+    o[6] = queued ? 1.0f : 0.0f; o[7] = any ? 1.0f : 0.0f;
+}
+// after k_shadow_prep: queued = 2 for the queries it left to k_shadow_bvh (the others it settled itself)
+__global__ void __launch_bounds__(256) k_probe_shadow_traversed(const uint32_t *squeue2, const Ctl *ctl, float *out) {
+    const uint32_t j = blockIdx.x*blockDim.x + threadIdx.x;
+    if (j < ctl->shadow_count2) out[8*size_t(squeue2[j] >> 2) + 6] = 2.0f;
+}
+// after k_shadow_bvh: vis and the finished lightF (NEE) / bsdfF (MIS) of each query
+__global__ void __launch_bounds__(128) k_probe_shadow_read(Scratch sr, const int *light_mis, float *out, uint32_t n) {
+    const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const bool mis = light_mis[2*size_t(i) + 1] != 0;
+    const float4 x = mis ? sr.M1[i] : sr.N1[i];
+    float *o = out + 8*size_t(i);
+    o[2] = float(sr.vis[2*size_t(i) + (mis ? 1 : 0)]); o[3] = x.x; o[4] = x.y; o[5] = x.z;
 }
 
 __global__ void __launch_bounds__(128) k_probe_choose_light(DScene sc, uint32_t seed, const uint32_t *pixel_id, uint32_t sample,

@@ -1026,6 +1026,30 @@ TGB_D bool light_hit_direct(const DScene &sc, const DPrim &l, V3 p, V3 d, float 
 TGB_D float mesh_direct_pdf(const DPrim &l, V3 p, V3 d, const Surface &ls) {
     return length_sq(p - ls.p)/(-dot(d, ls.Ng)*l.total_area);
 }
+// The shadow query of one NEE (mis = false: lightSample, TraceBase.cpp:246-285) or MIS (bsdfSample, :287-321) estimate towards
+// light l, as k_shade emits it; true when there is a query to trace.  f = the BSDF value (NEE) or sample weight (MIS), pdf = pdfL
+// (NEE) or the BSDF sample's pdf (MIS), pdf_b = NEE's BSDF pdf, dist = the sampled distance (NEE).
+//  * quad, cap and environment lights: the light's own hit is resolved here (light_hit_direct), lightF / bsdfF are finished into
+//    x.xyz and the query is a blocker test up to the light (any = true, t = its distance); none when the light is missed or
+//    emits nothing along d;
+//  * mesh lights: a closest-hit query that shadow_resolve_closest finishes: x = (f, pdfL) (NEE) or x.xyz = weight (MIS), t = the
+//    sampled distance (NEE) or the BSDF pdf (MIS).
+// The MIS query keeps x.w (NEE's pdfB shares that record).
+TGB_D bool light_query(const DScene &sc, const DPrim &l, V3 p, V3 d, float epsilon, bool mis, V3 f, float pdf, float pdf_b,
+                       float dist, float4 &x, float &t, bool &any) {
+    if (l.type == TGB_PRIM_MESH) {
+        any = false; x = make_float4(f.x, f.y, f.z, mis ? x.w : pdf); t = mis ? pdf : dist;
+        return true;
+    }
+    V3 em; float tfar, directPdf;
+    const bool hitL = light_hit_direct(sc, l, p, d, epsilon, mis ? -1.0f : dist, em, tfar, directPdf);
+    if (!hitL || is_zero(em)) return false;
+    V3 r;
+    if (mis) { r = em*f; r = r*power_heuristic(pdf, directPdf); }
+    else { r = (f*em)/pdf; r = r*power_heuristic(pdf, pdf_b); }
+    any = true; x = make_float4(r.x, r.y, r.z, mis ? x.w : 0.0f); t = tfar;
+    return true;
+}
 
 TGB_D float4 pack_hit(const Hit &h) { return make_float4(h.t, h.u, h.v, __int_as_float(h.id)); }
 TGB_D Hit unpack_hit(float4 v) { Hit h; h.t = v.x; h.u = v.y; h.v = v.z; h.id = __float_as_int(v.w); return h; }
@@ -1136,10 +1160,12 @@ __global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MI
 
 // Parity hook (tgb200_trace_closest): rays in AoS tgb_ray, hits out as tgb_hit, through the same analytic pass and
 // the same BVH traversal code as the renderer (global-memory nodes only).
+// Rays the analytic pass settled through the BVH's top-level cut are not in `list` (k_hook_analytic).
 struct HookPolicy {
-    const tgb_ray *rays; Hit *out; uint32_t i;
+    const tgb_ray *rays; Hit *out; const uint32_t *list, *count; uint32_t i;
     TGB_D bool fetch(uint32_t idx, V3 &o, V3 &d, float &tnear, Hit &h, bool &any) {
-        i = idx;
+        if (idx >= *count) return false;
+        i = list[idx];
         o = v3(rays[i].o[0], rays[i].o[1], rays[i].o[2]); d = v3(rays[i].d[0], rays[i].d[1], rays[i].d[2]); tnear = rays[i].tmin;
         h = out[i]; any = false;
         return true;
@@ -1147,23 +1173,31 @@ struct HookPolicy {
     TGB_D void finish(const Hit &h) { out[i] = h; }
     TGB_D int ignore() const { return -1; }
 };
-__global__ void __launch_bounds__(256) k_hook_analytic(DScene sc, const tgb_ray *rays, Hit *out, uint32_t n) {
+// The analytic part of each query, then (cut = 1) the BVH's top-level cut as k_accum applies it: a ray that misses every cut box
+// before its analytic hit is settled here; the others are listed for the BVH kernel.
+__global__ void __launch_bounds__(256) k_hook_analytic(DScene sc, const tgb_ray *rays, Hit *out, uint32_t n, int cut, uint32_t *list,
+                                                       uint32_t *count) {
     uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
     if (i >= n) return;
-    out[i] = analytic_closest(sc, v3(rays[i].o[0], rays[i].o[1], rays[i].o[2]), v3(rays[i].d[0], rays[i].d[1], rays[i].d[2]), rays[i].tmin, rays[i].tmax);
+    const V3 o = v3(rays[i].o[0], rays[i].o[1], rays[i].o[2]), d = v3(rays[i].d[0], rays[i].d[1], rays[i].d[2]);
+    const Hit h = analytic_closest(sc, o, d, rays[i].tmin, rays[i].tmax);
+    out[i] = h;
+    if (!cut || mesh_cut_hit(sc, o, d, rays[i].tmin, h.t)) list[atomicAdd(count, 1u)] = i;
 }
 template <bool CURVES>
-__global__ void __launch_bounds__(kTraceBlock) k_hook_bvh(DScene sc, const tgb_ray *rays, Hit *out, uint32_t n) {
+__global__ void __launch_bounds__(kTraceBlock) k_hook_bvh(DScene sc, const tgb_ray *rays, Hit *out, const uint32_t *list,
+                                                         const uint32_t *count, uint32_t n) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    HookPolicy pol; pol.rays = rays; pol.out = out; pol.i = 0;
+    HookPolicy pol; pol.rays = rays; pol.out = out; pol.list = list; pol.count = count; pol.i = 0;
     bvh_traverse_multi<CURVES>(sc, reinterpret_cast<int *>(smem_raw), pol, n);
 }
 // The same queries through the renderer's PERSISTENT kernel body (treelet staged in shared memory, lane refill): the
 // second half of the hit-id parity check, so the staged copy of the top nodes is pinned as well.
 struct HookPersistPolicy {
-    const tgb_ray *rays; Hit *out; uint32_t i;
+    const tgb_ray *rays; Hit *out; const uint32_t *list, *count; uint32_t i;
     TGB_D bool fetch(uint32_t idx, V3 &o, V3 &d, float &tnear, Hit &h, bool &any) {
-        i = idx;
+        if (idx >= *count) return false;
+        i = list[idx];
         o = v3(rays[i].o[0], rays[i].o[1], rays[i].o[2]); d = v3(rays[i].d[0], rays[i].d[1], rays[i].d[2]); tnear = rays[i].tmin;
         h = out[i]; any = false;
         return true;
@@ -1172,11 +1206,12 @@ struct HookPersistPolicy {
     TGB_D int ignore() const { return -1; }
 };
 template <bool CURVES>
-__global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_hook_persist(DScene sc, const tgb_ray *rays, Hit *out, uint32_t n, uint32_t *counter) {
+__global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_hook_persist(DScene sc, const tgb_ray *rays, Hit *out, const uint32_t *list,
+                                                                                          const uint32_t *count, uint32_t n, uint32_t *counter) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const uint4 *treelet = stage_treelet(sc, smem_raw);
     int *smem_stack = reinterpret_cast<int *>(smem_raw + size_t(sc.n_treelet)*64);
-    HookPersistPolicy pol; pol.rays = rays; pol.out = out; pol.i = 0;
+    HookPersistPolicy pol; pol.rays = rays; pol.out = out; pol.list = list; pol.count = count; pol.i = 0;
     bvh_traverse_persistent<CURVES>(sc, treelet, smem_stack, pol, n, counter);
 }
 __global__ void __launch_bounds__(256) k_hook_finish(DScene sc, const tgb_ray *rays, const Hit *in, tgb_hit *hits, uint32_t n) {
@@ -1394,19 +1429,8 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
                             V3 f = bsdf_eval<CURVES, LS>(sc, b, sf, e);
                             if (!is_zero(f)) {
                                 float pdfB = bsdf_pdf<CURVES, LS>(sc, b, sf, e);
-                                if (l.type == TGB_PRIM_MESH) {
-                                    qn = true; qn_any = false;
-                                    qnt = ls.dist; n1 = make_float4(f.x, f.y, f.z, ls.pdf); m1.w = pdfB;
-                                } else {
-                                    V3 em; float tfar, directPdf;
-                                    const bool hitL = light_hit_direct(sc, l, sf.p, ls.d, epsilon, ls.dist, em, tfar, directPdf);
-                                    if (hitL && !is_zero(em)) {
-                                        V3 lightF = (f*em)/ls.pdf;
-                                        lightF = lightF*power_heuristic(ls.pdf, pdfB);
-                                        qn = true; qn_any = true;
-                                        qnt = tfar; n1 = make_float4(lightF.x, lightF.y, lightF.z, 0.0f);
-                                    }
-                                }
+                                qn = light_query(sc, l, sf.p, ls.d, epsilon, false, f, ls.pdf, pdfB, ls.dist, n1, qnt, qn_any);
+                                m1.w = pdfB;
                                 if (qn) qnd = ls.d;
                             }
                         }
@@ -1419,19 +1443,7 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
                         if (set.enable_consistency_checks)
                             ok = (dot(wo, sf.Ng) < 0.0f) == ((e.wo.z < 0.0f) != e.flipped);
                         if (ok) {
-                            if (l.type == TGB_PRIM_MESH) {
-                                qm = true; qm_any = false;
-                                m1.x = e.weight.x; m1.y = e.weight.y; m1.z = e.weight.z; mpb = e.pdf;
-                            } else {
-                                V3 em; float tfar, directPdf;
-                                const bool hitL = light_hit_direct(sc, l, sf.p, wo, epsilon, -1.0f, em, tfar, directPdf);
-                                if (hitL && !is_zero(em)) {
-                                    V3 bsdfF = em*e.weight;
-                                    bsdfF = bsdfF*power_heuristic(e.pdf, directPdf);
-                                    qm = true; qm_any = true;
-                                    m1.x = bsdfF.x; m1.y = bsdfF.y; m1.z = bsdfF.z; mpb = tfar;
-                                }
-                            }
+                            qm = light_query(sc, l, sf.p, wo, epsilon, true, e.weight, e.pdf, 0.0f, -1.0f, m1, mpb, qm_any);
                             if (qm) { qmd = wo; qmt = mpb; }
                         }
                     }

@@ -52,6 +52,7 @@ def load():
     L.tgb200_bsdf_sample_probe.argtypes = [vp, u32, u32, vp, vp, u32, f32, f32, u32, i32, vp, vp, vp]
     L.tgb200_light_probe.argtypes = [vp, i32, u32, u32, u32, vp, vp]
     L.tgb200_choose_light_probe.argtypes = [vp, u32, u32, vp, u32, vp, vp]
+    L.tgb200_shadow_probe.argtypes = [vp, u32, vp, vp, vp]
     L.tgb200_destroy.argtypes = [vp]; L.tgb200_destroy.restype = None
     L.tgb200_last_error.argtypes = [vp]; L.tgb200_last_error.restype = C.c_char_p
     L.tgb200_abi_version.restype = u32

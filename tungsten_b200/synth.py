@@ -308,6 +308,30 @@ def cube_city(out_dir=None, name="cube_city", n=12, res=(128, 128), spp=16, max_
     return write_scene(out_dir, name, sc)
 
 
+def flush_lights(out_dir, name="flush_lights", res=(64, 64), spp=16, max_bounces=8):
+    """Cornell box with lights flush with a blocker, so that a shadow query finds a blocker at exactly the light's distance: a
+    table-top quad at y = 0.8 with two quad lights in its plane, one listed before the table and one after it, and a mesh shelf at
+    y = 1.4 with a mesh light in its plane.  All of them are unrotated (normal +y), so each pair's plane is the same float32 plane
+    and the hits of a ray on both are bit-identical ties."""
+    sv, st = grid_mesh(4, 4, 1.0)
+    lv, lt = grid_mesh(2, 2, 1.0)
+    meshes = {name + "_shelf.wo3": (sv, st), name + "_lamp.wo3": (lv, lt)}
+    bsdfs = [_lambert("table", [0.5, 0.45, 0.4]), {"name": "lamp", "type": "null", "albedo": 1.0}]
+
+    def flat(nm, bsdf, pos, scale, **kw):
+        d = {"name": nm, "type": "quad", "bsdf": bsdf, "transform": {"position": list(pos), "scale": list(scale)}}
+        d.update(kw); return d
+    prims = [flat("table", "table", (0.0, 0.8, 0.3), (1.2, 1, 1.0)),
+             flat("flush_after", "lamp", (0.3, 0.8, 0.35), (0.25, 1, 0.3), emission=[6.0, 5.0, 3.0]),
+             {"name": "shelf", "type": "mesh", "file": name + "_shelf.wo3", "smooth": False, "bsdf": "table",
+              "transform": {"position": [0.45, 1.4, -0.5], "scale": [0.8, 1.0, 0.6]}},
+             {"name": "mesh_lamp", "type": "mesh", "file": name + "_lamp.wo3", "smooth": False, "bsdf": "lamp",
+              "emission": [3.0, 4.0, 6.0], "transform": {"position": [0.45, 1.4, -0.5], "scale": [0.3, 1.0, 0.3]}}]
+    sc = cornell_box(res, spp, max_bounces, extra_bsdfs=bsdfs, extra_prims=prims, light_emission=(8, 6, 2))
+    sc["primitives"].insert(0, flat("flush_before", "lamp", (-0.25, 0.8, 0.3), (0.3, 1, 0.25), emission=[4.0, 6.0, 5.0]))
+    return write_scene(out_dir, name, sc, meshes)
+
+
 # ---- HDR environment maps ----------------------------------------------------------------------
 def save_rgbe(path, img):
     """Flat (non-RLE) Radiance .hdr writer; rows top-down ("-Y h +X w")."""
