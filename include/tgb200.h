@@ -274,11 +274,11 @@ int  tgb200_bvh_selftest(const float *tri_verts, uint32_t n, uint32_t *n_nodes, 
 /* Host-only: the hair BCSDF tables tgb200_create precomputes for one material (HairBcsdf.cpp:318-446): tables = 3 lobes
  * (R, TT, TRT) x 64 x 64 x RGB, sums = 3 x 64 row sums of the sampling weights, v = the three longitudinal variances. */
 int  tgb200_hair_selftest(float roughness, float scale_angle_deg, const float *sigma_a, float *tables, float *sums, float *v);
-/* Host-only check of the quantised device BVH (QNode4, 8-bit child boxes + shared-memory treelet image): walks it on the host
+/* Host-only check of the quantised device BVH (QNode4, 8-bit child boxes): walks it on the host
  * with the kernels' node arithmetic for n_rays rays (8 floats each: o, d, tmin, tmax) and compares the closest t with brute
  * force over all triangles, bit for bit.  *mismatches = rays that differ (must be 0).                                   */
-int  tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays, uint32_t max_treelet,
-                          uint32_t *mismatches, uint32_t *n_nodes, uint32_t *n_treelet, uint64_t *node_visits);
+int  tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays,
+                          uint32_t *mismatches, uint32_t *n_nodes, uint64_t *node_visits);
 /* Test hooks: each launches one kernel on the context's stream that calls the device functions the shading kernel calls, on
  * host arrays in and out.  A NULL context returns TGB_ERR_INVALID.
  * tgb200_bsdf_probe: Bsdf::eval(event, adjoint=false) rgb + Bsdf::pdf of bsdf `bsdf` for n (wi, wo) pairs in the local frame

@@ -199,50 +199,18 @@ static void build_from_boxes(std::vector<Box> &tb, std::vector<float> &cent, uin
 }
 
 // ---- quantised layout -------------------------------------------------------------------------------------------
-namespace {
-inline float node_half_area(const Node4 &nd, int k) {
-    float dx = nd.f[4 + k] - nd.f[k], dy = nd.f[12 + k] - nd.f[8 + k], dz = nd.f[20 + k] - nd.f[16 + k];
-    return dx*dy + dy*dz + dz*dx;
-}
-}  // namespace
-
-void quantize_bvh4(const Bvh4 &in, uint32_t max_treelet, QBvh4 &out, int32_t empty_link) {
-    out.nodes.clear(); out.old_index.clear(); out.treelet_image.clear(); out.n_treelet = 0;
+void quantize_bvh4(const Bvh4 &in, QBvh4 &out, int32_t empty_link) {
+    out.nodes.clear(); out.old_index.clear();
     const size_t n = in.nodes.size();
     if (n == 0) return;
-    // ---- order: treelet = repeatedly take the open inner node with the largest surface area (the nodes a random ray is
-    // most likely to visit), parents before children; the rest depth-first under each treelet frontier node.
+    // order: depth-first from the root, children 0..3 in order (pushed 3..0)
     std::vector<int32_t> order; order.reserve(n);
-    std::vector<uint8_t> taken(n, 0);
-    {
-        struct Open { float area; int32_t node; };
-        auto cmp = [](const Open &a, const Open &b) { return a.area < b.area || (a.area == b.area && a.node > b.node); };
-        std::vector<Open> heap; heap.push_back({std::numeric_limits<float>::infinity(), 0});
-        while (!heap.empty() && order.size() < size_t(max_treelet)) {
-            std::pop_heap(heap.begin(), heap.end(), cmp);
-            Open o = heap.back(); heap.pop_back();
-            order.push_back(o.node); taken[size_t(o.node)] = 1;
-            const Node4 &nd = in.nodes[size_t(o.node)];
-            for (int k = 0; k < 4; ++k) if (nd.link[k] >= 0) { heap.push_back({node_half_area(nd, k), nd.link[k]}); std::push_heap(heap.begin(), heap.end(), cmp); }
-        }
-        out.n_treelet = uint32_t(order.size());
-        // remaining nodes: depth-first from every frontier node, in treelet order (children near their parents)
-        std::vector<int32_t> stack;
-        auto dfs = [&](int32_t root) {
-            stack.clear(); stack.push_back(root);
-            while (!stack.empty()) {
-                int32_t x = stack.back(); stack.pop_back();
-                if (taken[size_t(x)]) continue;
-                taken[size_t(x)] = 1; order.push_back(x);
-                const Node4 &nd = in.nodes[size_t(x)];
-                for (int k = 3; k >= 0; --k) if (nd.link[k] >= 0) stack.push_back(nd.link[k]);
-            }
-        };
-        if (out.n_treelet == 0) dfs(0);
-        for (uint32_t i = 0; i < out.n_treelet; ++i) {
-            const Node4 &nd = in.nodes[size_t(order[i])];
-            for (int k = 0; k < 4; ++k) if (nd.link[k] >= 0 && !taken[size_t(nd.link[k])]) dfs(nd.link[k]);
-        }
+    std::vector<int32_t> stack(1, 0);
+    while (!stack.empty()) {
+        const int32_t x = stack.back(); stack.pop_back();
+        order.push_back(x);
+        const Node4 &nd = in.nodes[size_t(x)];
+        for (int k = 3; k >= 0; --k) if (nd.link[k] >= 0) stack.push_back(nd.link[k]);
     }
     std::vector<int32_t> new_index(n, -1);
     for (size_t i = 0; i < order.size(); ++i) new_index[size_t(order[i])] = int32_t(i);
@@ -284,16 +252,10 @@ void quantize_bvh4(const Bvh4 &in, uint32_t max_treelet, QBvh4 &out, int32_t emp
         for (int k = 0; k < 4; ++k) q.link[k] = nd.link[k] >= 0 ? new_index[size_t(nd.link[k])] : (nd.link[k] == kEmptyLink ? empty_link : nd.link[k]);
         out.nodes[i] = q;
     }
-    out.treelet_image.resize(out.n_treelet);
-    for (uint32_t i = 0; i < out.n_treelet; ++i) {
-        const uint32_t *src = reinterpret_cast<const uint32_t *>(&out.nodes[i]);
-        uint32_t *dst = reinterpret_cast<uint32_t *>(&out.treelet_image[i]);
-        for (uint32_t c = 0; c < 4; ++c) std::memcpy(dst + 4*(c ^ ((i >> 1) & 3u)), src + 4*c, 16);
-    }
 }
 
 void qnode_slab_host(const QNode4 &nd, const float o[3], const float inv_d[3], float tnear, float tfar, float t_out[4]) {
-    // mirrors Traversal::visit_loaded in tgb_wavefront.cuh operation for operation (fmaf = one rounding, as FFMA)
+    // mirrors Traversal::visit in tgb_wavefront.cuh operation for operation (fmaf = one rounding, as FFMA)
     const float org[3] = {nd.ox, nd.oy, nd.oz}, S[3] = {nd.sx, nd.sy, nd.sz};
     const uint32_t lo[3] = {nd.lox, nd.loy, nd.loz}, hi[3] = {nd.hix, nd.hiy, nd.hiz};
     float a[3], b[3]; uint32_t nearw[3], farw[3];

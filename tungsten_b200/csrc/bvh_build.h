@@ -53,17 +53,14 @@ struct alignas(64) QNode4 {
 static_assert(sizeof(QNode4) == 64, "QNode4 layout");
 
 struct QBvh4 {
-    std::vector<QNode4> nodes;        // renumbered: [0, n_treelet) = the top treelet (largest surface area first), rest depth-first
+    std::vector<QNode4> nodes;        // renumbered depth-first from the root
     std::vector<int32_t> old_index;   // new index -> index in the Node4 array it was made from
-    uint32_t n_treelet = 0;
-    std::vector<QNode4> treelet_image;   // the first n_treelet nodes with their 16-byte chunks XOR-swizzled for shared memory:
-                                         // chunk c of node i sits at chunk c ^ ((i >> 1) & 3)  (conflict-free-ish LDS.128)
 };
-// Quantise `in` (float 4-ary BVH) into `out`; at most max_treelet nodes go to the treelet (0 = none).
+// Quantise `in` (float 4-ary BVH) into `out`.
 // Empty child slots get the inverted box (lo 255, hi 0), which no ray can enter, and `empty_link` instead of kEmptyLink: the
 // kernels do not test for empty slots, so the link must be harmless to follow (the caller passes a one-primitive leaf that
 // holds an all-zero record, which every primitive test rejects).
-void quantize_bvh4(const Bvh4 &in, uint32_t max_treelet, QBvh4 &out, int32_t empty_link = kEmptyLink);
+void quantize_bvh4(const Bvh4 &in, QBvh4 &out, int32_t empty_link = kEmptyLink);
 // Host evaluation of one node visit with the kernels' arithmetic (tests + tgb200_qbvh_selftest): entry distance of the
 // four children for the ray (o, 1/d), INFINITY where the slab test fails.
 void qnode_slab_host(const QNode4 &nd, const float o[3], const float inv_d[3], float tnear, float tfar, float t_out[4]);

@@ -61,8 +61,6 @@ struct tgb_ctx {
     Scratch sr{};                   // per-bounce scratch records + per-step results
     uint32_t *order = nullptr, *squeue = nullptr, *squeue2 = nullptr;   // ray-coherence visiting order of k_trace; shadow-query queues (emitted / left after the analytic pass)
     uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels
-    size_t trace_smem = 0;          // their dynamic shared memory: treelet image + stacks + mbarrier
-    size_t l2_window_bytes = 0;     // bytes of BVH data pinned in L2 through the stream's access-policy window (0 = none)
     bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
     bool has_curves = false;        // selects the kernel instantiations with the curve-segment test and per-hit epsilon
@@ -651,31 +649,11 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         tri_isect[3*k + 1] = make_float4(e1.y, e1.z, e2.x, e2.y);
         tri_isect[3*k + 2] = make_float4(e2.z, ng.x, ng.y, ng.z);
     }
-    // device node layout: QNode4 (64 B, 8-bit child boxes on a per-node grid), renumbered so that the nodes a random ray is most
-    // likely to visit come first: those are bulk-copied into shared memory by every traversal CTA (the "treelet")
-    QBvh4 qb;
-    {
-        // shared-memory budget of one traversal CTA: 227 KB / resident CTAs - stacks - 1 KB system reserve
-        const long budget = long(227*1024)/TGB_MINB - long(kStackSmemBytes) - 1024 - 16;
-        // Measured on C1 (B200, and again on an H100: 5 % slower): staging the top 320 nodes costs more than it saves (the carve-out shrinks L1 and lowers its hit rate,
-        // and the treelet branch adds instructions to a kernel that is ALU-issue bound), so the treelet is opt-in:
-        // TGB_TREELET=<nodes> (capped by the budget above).
-        long want = 0;
-        if (const char *e = getenv("TGB_TREELET")) want = std::min(std::max(0L, budget/64), std::max(0L, atol(e)));
-#if !TGB_QNODES
-        want = 0;
-#endif
-        // empty child slots link to a one-triangle leaf holding the all-zero record behind the last primitive (den == 0: rejected)
-        const int32_t empty_link = ~int32_t(uint32_t(btris.size() + cboxes.size()) << 3);
-        quantize_bvh4(bvh, uint32_t(want), qb, empty_link);
-    }
-#if TGB_QNODES
-    std::vector<float4> nodes;                                  // float nodes stay on the host (cut construction above)
-#else
-    std::vector<float4> nodes(8*bvh.nodes.size());
-    std::memcpy(nodes.data(), bvh.nodes.data(), bvh.nodes.size()*sizeof(Node4));
-#endif
-    c->geom_bytes = nodes.size()*16 + qb.nodes.size()*sizeof(QNode4) + tri_isect.size()*16 + tri_shade.size()*16 + bvh.order.size()*8;
+    // device node layout: QNode4 (64 B, 8-bit child boxes on a per-node grid)
+    // empty child slots link to a one-triangle leaf holding the all-zero record behind the last primitive (den == 0: rejected)
+    const int32_t empty_link = ~int32_t(uint32_t(btris.size() + cboxes.size()) << 3);
+    QBvh4 qb; quantize_bvh4(bvh, qb, empty_link);
+    c->geom_bytes = qb.nodes.size()*sizeof(QNode4) + tri_isect.size()*16 + tri_shade.size()*16 + bvh.order.size()*8;
 
     int rc;
     if ((rc = dev_upload(c, &sc.prims, prims))) return rc;
@@ -697,44 +675,11 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         for (size_t k = 0; k < btris.size(); ++k) std::memcpy(&shade_leaf[4*k], &tri_shade[4*size_t(bvh.order[k])], 4*sizeof(float4));
         if ((rc = dev_upload(c, &sc.tri_shade, shade_leaf))) return rc;
     }
-    {   // BVH nodes + intersection records in ONE allocation, so that a single L2 access-policy window can pin them.
-        // The traversal kernels re-read this working set (C1: 78 MB) for every wavefront while ~1.4 GB of path state streams
-        // through the same L2 in between, so k_trace moves several times its algorithmic DRAM bytes.  On the previous GPU
-        // (B200, 126 MB L2, where the working set fits) the window gained little in k_trace, which is not waiting on DRAM, and
-        // the streaming kernels lost more to the carved-out L2, so the window is opt-in: TGB_L2_PERSIST=1.  Not measured on
-        // the H100, whose 50 MB L2 the working set exceeds: the trade-off there may differ.
-        size_t fb = nodes.size()*sizeof(float4), qbytes = qb.nodes.size()*sizeof(QNode4), tb = tri_isect.size()*sizeof(float4);
-        size_t fb_al = (fb + 255) & ~size_t(255), qb_al = (qbytes + 255) & ~size_t(255);
-        size_t nb = fb_al + qbytes, nb_al = fb_al + qb_al;
-        char *slab = nullptr;
-        if ((rc = dev_alloc(c, &slab, nb_al + std::max<size_t>(tb, 16)))) return rc;
-        if (fb) CU(cudaMemcpy(slab, nodes.data(), fb, cudaMemcpyHostToDevice));
-        if (qbytes) CU(cudaMemcpy(slab + fb_al, qb.nodes.data(), qbytes, cudaMemcpyHostToDevice));
-        if (tb) CU(cudaMemcpy(slab + nb_al, tri_isect.data(), tb, cudaMemcpyHostToDevice));
-        sc.nodes = reinterpret_cast<const float4 *>(slab); sc.qnodes = reinterpret_cast<const uint4 *>(slab + fb_al);
-        sc.tri_isect = reinterpret_cast<const float4 *>(slab + nb_al);
-        sc.n_treelet = qb.n_treelet; sc.treelet_img = nullptr; sc.qy = 0x3F80u;
-        if (qb.n_treelet) {
-            QNode4 *img = nullptr;
-            if ((rc = dev_alloc(c, &img, qb.treelet_image.size()))) return rc;
-            CU(cudaMemcpy(img, qb.treelet_image.data(), qb.treelet_image.size()*sizeof(QNode4), cudaMemcpyHostToDevice));
-            sc.treelet_img = reinterpret_cast<const uint4 *>(img);
-        }
-        const char *env = getenv("TGB_L2_PERSIST");
-        if (nb + tb > 0 && env && env[0] == '1') {
-            cudaDeviceProp prop; CU(cudaGetDeviceProperties(&prop, c->device));
-            size_t window = std::min<size_t>(nb_al + tb, size_t(prop.accessPolicyMaxWindowSize));
-            size_t carve = std::min<size_t>(window, size_t(prop.persistingL2CacheMaxSize));
-            if (window && carve && cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve) == cudaSuccess) {
-                cudaStreamAttrValue attr; std::memset(&attr, 0, sizeof(attr));
-                attr.accessPolicyWindow.base_ptr = slab; attr.accessPolicyWindow.num_bytes = window;
-                attr.accessPolicyWindow.hitRatio = float(std::min(1.0, double(carve)/double(window)));
-                attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-                attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-                if (cudaStreamSetAttribute(c->stream, cudaStreamAttributeAccessPolicyWindow, &attr) == cudaSuccess) c->l2_window_bytes = carve;
-            }
-            cudaGetLastError();
-        }
+    if ((rc = dev_upload(c, &sc.tri_isect, tri_isect))) return rc;
+    {
+        const QNode4 *qn = nullptr;
+        if ((rc = dev_upload(c, &qn, qb.nodes))) return rc;
+        sc.qnodes = reinterpret_cast<const uint4 *>(qn); sc.qy = 0x3F80u;
     }
     std::vector<uint32_t> sobol(1024*32);
     std::memcpy(sobol.data(), tgb_sobol_blob, sobol.size()*4);
@@ -867,8 +812,8 @@ void enqueue_iteration(tgb_ctx *c, const BatchInfo &bi, int cur, uint32_t bound,
     if (prof) cudaEventRecord(c->ev_k[slot][1], st);
     if (has_bvh) {
         uint32_t grid = std::min(blocks(bound, kTraceBlock), c->persist_blocks);
-        if (curves) k_trace<true><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, pb, c->order, c->ctl);
-        else k_trace<false><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, pb, c->order, c->ctl);
+        if (curves) k_trace<true><<<grid, kTraceBlock, 0, st>>>(sc, pb, c->order, c->ctl);
+        else k_trace<false><<<grid, kTraceBlock, 0, st>>>(sc, pb, c->order, c->ctl);
         launches++;
     }
     if (prof) cudaEventRecord(c->ev_k[slot][2], st);
@@ -888,8 +833,8 @@ void enqueue_iteration(tgb_ctx *c, const BatchInfo &bi, int cur, uint32_t bound,
     if (prof) cudaEventRecord(c->ev_k[slot][4], st);
     if (has_bvh) {
         uint32_t grid = std::min(blocks(2*bound, kTraceBlock), c->persist_blocks);
-        if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
-        else k_shadow_bvh<false><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
+        if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
+        else k_shadow_bvh<false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
         launches++;
     }
     if (prof) cudaEventRecord(c->ev_k[slot][5], st);
@@ -1127,7 +1072,6 @@ void tgb200_destroy(tgb_ctx *c) {
     }
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
-    if (c->l2_window_bytes) cudaCtxResetPersistingL2Cache();
     for (void *p : c->allocs) cudaFree(p);
     if (c->sr.R) cudaFree(c->sr.R);
     if (c->h_ctl) cudaFreeHost(c->h_ctl);
@@ -1218,17 +1162,15 @@ static int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
         if ((rc = alloc_wavefront(c, cap))) break;
         {   // persistent traversal grid = twice what is resident at once (blocks per SM x SMs, smaller of the two kernels): the
             // second wave evens out the end of a launch
-            c->trace_smem = trace_smem_bytes(c->sc.n_treelet);
             int sms = 0, b1 = 0, b2 = 0;
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             cudaError_t e = cudaSuccess;
             auto prep = [&](auto kern, int *nb) {
-                if (e == cudaSuccess) e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(c->trace_smem));
-                if (e == cudaSuccess && nb) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(nb, kern, kTraceBlock, c->trace_smem);
+                if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(nb, kern, kTraceBlock, 0);
             };
-            if (c->has_curves) { prep(k_trace<true>, &b1); prep(k_shadow_bvh<true>, &b2); prep(k_hook_persist<true>, nullptr); }
-            else { prep(k_trace<false>, &b1); prep(k_shadow_bvh<false>, &b2); prep(k_hook_persist<false>, nullptr); }
-            if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s; %zu B of shared memory per block)", cudaGetErrorString(e), c->trace_smem); break; }
+            if (c->has_curves) { prep(k_trace<true>, &b1); prep(k_shadow_bvh<true>, &b2); }
+            else { prep(k_trace<false>, &b1); prep(k_shadow_bvh<false>, &b2); }
+            if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
             const char *mult = getenv("TGB_PERSIST_MULT");
             c->persist_blocks = uint32_t(sms*std::min(b1, b2))*uint32_t(mult ? std::max(1, atoi(mult)) : 2);
         }
@@ -1332,19 +1274,12 @@ static cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t
         c->stats.kernel_launches++;
     }
     if (e == cudaSuccess && c->sc.n_nodes) {
-        // the renderer's own persistent kernel body: treelet staged in shared memory, lane refill (TGB_HOOK_SIMPLE=1: one ray
-        // per thread, nodes from global memory only)
-        const char *simple = getenv("TGB_HOOK_SIMPLE");
-        if (simple && simple[0] == '1') {
-            if (c->has_curves) k_hook_bvh<true><<<blocks(n, kTraceBlock), kTraceBlock, kStackSmemBytes, c->stream>>>(c->sc, dr, dx, list + 1, list, n);
-            else k_hook_bvh<false><<<blocks(n, kTraceBlock), kTraceBlock, kStackSmemBytes, c->stream>>>(c->sc, dr, dx, list + 1, list, n);
-        } else {
-            e = cudaMemsetAsync(&c->ctl->cursor_trace, 0, sizeof(uint32_t), c->stream);
-            uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
-            if (e == cudaSuccess) {
-                if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, c->trace_smem, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
-                else k_hook_persist<false><<<grid, kTraceBlock, c->trace_smem, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
-            }
+        // the renderer's own persistent kernel body (lane refill)
+        e = cudaMemsetAsync(&c->ctl->cursor_trace, 0, sizeof(uint32_t), c->stream);
+        uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
+        if (e == cudaSuccess) {
+            if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
+            else k_hook_persist<false><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
         }
         c->stats.kernel_launches++;
     }
@@ -1685,12 +1620,12 @@ int tgb200_generate_work(tgb_sample_record *records, uint32_t res_x, uint32_t re
 }
 
 // Host-only check of the quantised device BVH (no GPU needed): builds the 4-ary SAH tree over n triangles exactly as
-// tgb200_create does (same padding), quantises it (QNode4 + treelet), and walks it on the HOST with the kernels' node
+// tgb200_create does (same padding), quantises it (QNode4), and walks it on the HOST with the kernels' node
 // arithmetic (qnode_slab_host mirrors Traversal::visit) and their triangle test for every ray (8 floats: o, d, tmin, tmax).
 // The closest t must equal the brute-force closest t over all triangles bit for bit (ids may differ only on exact ties).
-// Returns the number of rays whose t differs in *mismatches; also verifies the swizzled treelet image and the link remap.
-int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays, uint32_t max_treelet,
-                         uint32_t *mismatches, uint32_t *n_nodes, uint32_t *n_treelet, uint64_t *node_visits) {
+// Returns the number of rays whose t differs in *mismatches; also verifies the link remap.
+int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays,
+                         uint32_t *mismatches, uint32_t *n_nodes, uint64_t *node_visits) {
     if ((n && !tri_verts) || (n_rays && !rays) || !mismatches) return TGB_ERR_INVALID;
     std::vector<BuildTri> tris(n);
     float extent = 0.0f;
@@ -1698,14 +1633,9 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
     for (uint32_t r = 0; r < n_rays; ++r) for (int k = 0; k < 3; ++k) extent = std::max(extent, std::fabs(rays[8*size_t(r) + k]));
     Bvh4 bvh; build_bvh4(tris.data(), n, bvh, 0, 1e-6f*extent, 4, 0.5f);
     const int32_t empty_link = ~int32_t(n << 3);                       // a leaf past the last triangle (the walk below skips it)
-    QBvh4 qb; quantize_bvh4(bvh, max_treelet, qb, empty_link);
+    QBvh4 qb; quantize_bvh4(bvh, qb, empty_link);
     if (n_nodes) *n_nodes = uint32_t(qb.nodes.size());
-    if (n_treelet) *n_treelet = qb.n_treelet;
-    if (qb.nodes.size() != bvh.nodes.size() || qb.n_treelet > qb.nodes.size() || qb.treelet_image.size() != qb.n_treelet) return TGB_ERR_INVALID;
-    for (uint32_t i = 0; i < qb.n_treelet; ++i) {                       // un-swizzling the image gives the nodes back
-        const uint32_t *img = reinterpret_cast<const uint32_t *>(&qb.treelet_image[i]), *nd = reinterpret_cast<const uint32_t *>(&qb.nodes[i]);
-        for (uint32_t cch = 0; cch < 4; ++cch) if (std::memcmp(img + 4*(cch ^ ((i >> 1) & 3u)), nd + 4*cch, 16) != 0) return TGB_ERR_INVALID;
-    }
+    if (qb.nodes.size() != bvh.nodes.size()) return TGB_ERR_INVALID;
     for (size_t i = 0; i < qb.nodes.size(); ++i) {                      // links: same leaves, children remapped consistently
         const Node4 &src = bvh.nodes[size_t(qb.old_index[i])];
         for (int k = 0; k < 4; ++k) {
@@ -1714,7 +1644,7 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
             else if (l < 0 || size_t(l) >= qb.nodes.size() || qb.old_index[size_t(l)] != src.link[k]) return TGB_ERR_INVALID;
         }
     }
-    auto tri_test = [&](uint32_t t, const V3 &o, const V3 &d, float tnear, float &best) {   // Traversal::run's triangle test
+    auto tri_test = [&](uint32_t t, const V3 &o, const V3 &d, float tnear, float &best) {   // Traversal::triangle
         V3 v0 = f3(tris[t].v0), v1 = f3(tris[t].v1), v2 = f3(tris[t].v2);
         V3 e1 = v0 - v1, e2 = v2 - v0, ng = cross(e1, e2);
         V3 C = v0 - o, R = cross(d, C);
@@ -1914,8 +1844,8 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
         k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(c->squeue2, c->ctl, dout + 8*size_t(off));
         if (sc.n_nodes) {
             const uint32_t grid = std::min(blocks(m, kTraceBlock), c->persist_blocks);
-            if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
-            else k_shadow_bvh<false><<<grid, kTraceBlock, c->trace_smem, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
+            if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
+            else k_shadow_bvh<false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
         }
         k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(c->sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
         e = cudaGetLastError();

@@ -125,17 +125,17 @@ struct DScene {
     // triangles: intersection records in BVH leaf order (3 x float4 each), leaf order -> global id,
     // global id -> primitive, shading records ALSO in leaf order (4 x float4 each: 3 normals, 3 uvs, material | primitive << 10)
     const float4 *tri_isect; const uint32_t *tri_global; const uint32_t *tri_prim; const float4 *tri_shade;
-    const float4 *nodes; uint32_t n_nodes; uint32_t n_tris;          // float Node4 array (128 B per node; only read by TGB_QNODES=0 builds)
-    // quantised nodes (QNode4, 64 B = 4 x uint4, bvh_build.h) in treelet-first order, and the swizzled image of the first
-    // n_treelet of them that the traversal kernels bulk-copy into shared memory
-    const uint4 *qnodes; const uint4 *treelet_img; uint32_t n_treelet;
+    uint32_t n_nodes; uint32_t n_tris;
+    // quantised nodes (QNode4, 64 B = 4 x uint4, bvh_build.h), depth-first from the root
+    const uint4 *qnodes;
     uint32_t qy;                // = 0x3F80: the constant bytes of 1 + q*2^-15 (see qplane in tgb_wavefront.cuh)
     // curve segments share the arrays above: records n_tris.. of tri_isect hold a segment's three nodes (x, y, z, width),
     // tri_global / tri_prim continue with global ids n_tris + segment
     uint32_t n_curve_segs;          // BVH primitives for curves = kCurvePieces sub-ranges per segment
     // "cut": <= 16 boxes of the BVH's top levels that together cover every triangle (same padded boxes the nodes hold).
     // A ray that misses all of them is answered by the kernel that creates it and never reaches a traversal kernel.
-    int n_cut; float cut[6][16];        // lo.x, hi.x, lo.y, hi.y, lo.z, hi.z
+    // (8-byte aligned: mesh_cut_hit reads two boxes' planes per 64-bit load from the kernel parameters)
+    int n_cut; alignas(8) float cut[6][16];        // lo.x, hi.x, lo.y, hi.y, lo.z, hi.z
     V3 bin_lo, bin_inv;         // ray-binning grid over the scene bounds: cell = (o - bin_lo)*bin_inv, 16 cells per axis
     const uint32_t *sobol;      // 1024 x 32 direction matrices
 };

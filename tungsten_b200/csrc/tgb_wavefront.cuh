@@ -3,8 +3,7 @@
 //                    paths that replace finished ones (appended behind the compacted survivors)
 //   k_trace        : TraceableScene::intersect (closest hit): persistent CTAs pull rays from the coherence-sorted queue and walk
 //                    the 4-ary BVH of 64-byte quantised nodes over all mesh triangles (+ curve segments, + the analytic
-//                    primitives when they are many) as a warp state machine (machine_traverse_persistent); optionally the
-//                    top of the tree is staged in shared memory by one bulk-async copy (TMA engine, mbarrier; off by default).
+//                    primitives when they are many) as a warp state machine (bvh_traverse_persistent).
 //                    Few analytic primitives are tested by the kernel that creates the ray instead
 //   k_shade        : makeLocalScatterEvent + handleSurface (NEE/MIS query generation, emission, BSDF sample, Russian roulette);
 //                    instantiations: material-sorted window, all-Lambert lobe set, curves
@@ -257,17 +256,10 @@ TGB_D bool curve_point_on_spline(float4 p0, float4 p1, float4 p2, float tMin, fl
 #ifndef TGB_MINB
 #define TGB_MINB 6
 #endif
-// node layout the traversal reads: 1 = QNode4 (64 B, 8-bit child boxes, 4 x LDG.128 per visit), 0 = float Node4 (128 B, 7 loads)
-#ifndef TGB_QNODES
-#define TGB_QNODES 1
-#endif
 constexpr int kTraceBlock = TGB_TRACE_BLOCK;
 constexpr int kSmemStack = TGB_SMEM_STACK;
 constexpr int kStackSize = 80;
 constexpr int kLocalStack = kStackSize - kSmemStack;
-constexpr size_t kStackSmemBytes = size_t(kSmemStack)*kTraceBlock*sizeof(int);
-// dynamic shared memory of a traversal kernel: [treelet image: n_treelet x 64 B][stack][mbarrier]
-TGB_HD size_t trace_smem_bytes(uint32_t n_treelet) { return size_t(n_treelet)*64 + kStackSmemBytes + 16; }
 
 TGB_D uint32_t smem_addr(const void *p) { return uint32_t(__cvta_generic_to_shared(p)); }
 // The stack pointer lives in a plain register variable next to this struct (a member would be spilled with the array).
@@ -287,41 +279,8 @@ struct TravStack {
     }
 };
 
-// ---- bulk-async staging of the top treelet (cp.async.bulk + mbarrier: the TMA engine copies, no thread touches the data) ----
-TGB_D void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_addr(bar)), "r"(count) : "memory");
-}
-TGB_D void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-TGB_D void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_addr(bar)), "r"(bytes) : "memory");
-}
-TGB_D void bulk_copy_g2s(void *dst_smem, const void *src_gmem, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smem_addr(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_addr(bar)) : "memory");
-}
-TGB_D void mbar_wait(uint64_t *bar, uint32_t parity) {
-    asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
-                 :: "r"(smem_addr(bar)), "r"(parity) : "memory");
-}
-// Called by every thread of a traversal CTA before its first node visit; returns the treelet's shared-memory image.
-// Thread 0 arms the barrier with the byte count and issues the copies (<= 32 KB each); all threads wait on phase 0.
-TGB_D const uint4 *stage_treelet(const DScene &sc, unsigned char *smem_raw) {
-    const uint32_t bytes = sc.n_treelet*64u;
-    if (bytes == 0) return nullptr;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(smem_raw + bytes + kStackSmemBytes);
-    if (threadIdx.x == 0) { mbar_init(bar, 1); fence_mbar_init(); }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(bar, bytes);
-        const unsigned char *src = reinterpret_cast<const unsigned char *>(sc.treelet_img);
-        for (uint32_t off = 0; off < bytes; off += 32768u) bulk_copy_g2s(smem_raw + off, src + off, min(32768u, bytes - off), bar);
-    }
-    mbar_wait(bar, 0);
-    return reinterpret_cast<const uint4 *>(smem_raw);
-}
-
-// BVH traversal over the mesh triangles: one ray per thread, per-lane while-while over the 4-ary BVH.
-// Node visit (QNode4, bvh_build.h) = 4 x 16-byte loads -- from the shared-memory treelet for the top nodes, else global --,
+// BVH traversal over the mesh triangles: one ray per lane over the 4-ary BVH.
+// Node visit (QNode4, bvh_build.h) = 4 x 16-byte loads from global memory,
 // per axis a = S/d, b = (origin - o)/d - a once per node, then per child plane ONE byte permute (1 + q*2^-15 assembled
 // straight into float bits) and ONE fma; the hit children are ordered near-to-far with a 5-exchange sorting network, the
 // nearest is entered and the others are pushed far-to-near (three predicated shared-memory stores).
@@ -330,6 +289,11 @@ TGB_D const uint4 *stage_treelet(const DScene &sc, unsigned char *smem_raw) {
 // `any`: occlusion query, stop at the first triangle hit.
 // Alternatives measured and rejected (B200): warp-synchronous speculative
 // traversal, if-if state machines with and without several rays per lane, 32-byte quantised BINARY nodes, higher occupancy.
+// Measured, lost and removed: the top nodes staged in shared memory by a bulk-async copy (H100, C1: 459 vs 486 Msamples/s);
+// (B200) an L2 persistence window over nodes + triangle records (little gain in k_trace, a loss in the streaming kernels),
+// 128-byte float nodes (7 dependent loads per visit against 4), a per-lane while-while walk (slower than the state machine),
+// the whole leaf or one triangle per LEAF trip instead of two, a triangle record or a node fetched one trip ahead (+12 / +16
+// registers, no gain), several rays reserved per atomicAdd.
 #define TGB_CSWAP(ta, la, tb, lb) { bool sw_ = tb < ta; float tt_ = sw_ ? tb : ta; tb = sw_ ? ta : tb; ta = tt_; \
                                     int ll_ = sw_ ? lb : la; lb = sw_ ? la : lb; la = ll_; }
 // 1 + q*2^-15 for byte K of word W: result bytes (0x3F, 0x80, q, 0x00).  The selector is an immediate and the constant word
@@ -346,12 +310,11 @@ template <int K> TGB_D float qplane(uint32_t w, uint32_t y) {
 #define TGB_QF(W, K) qplane<K>(W, qy)
 // CURVES: leaves whose code has bit 2 set hold curve segments (three float4 nodes per record, stored after the triangles);
 // a curve hit keeps (t, position along the segment, interpolated width) in (t, u, v) and id >= n_tris.
-// The traversal is a resumable object: run() walks until the ray is finished (true) or until `yield()` asks for a pause
-// after a leaf (false) -- the persistent kernels pause to hand new rays to the lanes whose ray has finished.
+// One lane's ray and its node / primitive tests; bvh_traverse_persistent drives it.
 template <bool CURVES>
 struct Traversal {
     V3 o, d; float tnear; bool any; Hit h;
-    float idx, idy, idz, oodx, oody, oodz; int nx, ny, nz, fx, fy, fz;
+    float idx, idy, idz, oodx, oody, oodz; int nx, ny, nz;
     CurveFrame cf; int last_seg; int cur;
     int ignore;         // analytic primitive an occlusion query must not count (the light it is aimed at), -1 = none
     // (the stack is a separate object: its dynamically indexed spill array would drag this whole struct into local memory)
@@ -366,44 +329,15 @@ struct Traversal {
         // The entry plane of a slab is its lo plane when the direction component is positive, else its hi plane (fma is
         // monotone, so this IS min(a, b) / max(a, b) of the two plane distances): pick which to read per axis once per ray.
         nx = idx < 0.0f ? 1 : 0; ny = idy < 0.0f ? 3 : 2; nz = idz < 0.0f ? 5 : 4;
-        fx = nx ^ 1; fy = ny ^ 1; fz = nz ^ 1;
         last_seg = -1; ignore = -1;
         if (CURVES) cf = curve_frame(d);
         cur = 0;
     }
 
     // one node visit: entry distances of the four children (INFINITY = culled) and their links
-    TGB_D void visit(const DScene &sc, const uint4 *treelet, float &t0, float &t1, float &t2, float &t3, int4 &lk) {
-#if TGB_QNODES
-        uint4 c0, c1, c2;
-        if (uint32_t(cur) < sc.n_treelet && treelet) {
-            const uint4 *nd = treelet + 4*cur; const int sw = (cur >> 1) & 3;
-            c0 = nd[sw]; c1 = nd[1 ^ sw]; c2 = nd[2 ^ sw]; const uint4 l = nd[3 ^ sw];
-            lk = make_int4(int(l.x), int(l.y), int(l.z), int(l.w));
-        } else {
-            const uint4 *nd = sc.qnodes + 4*size_t(cur);
-            c0 = __ldg(nd); c1 = __ldg(nd + 1); c2 = __ldg(nd + 2); lk = __ldg(reinterpret_cast<const int4 *>(nd + 3));
-        }
-        visit_loaded(sc, c0, c1, c2, lk, t0, t1, t2, t3);
-#else
-        const int EMPTY = int(0x80000000u);
-        const float4 *nd = sc.nodes + 8*size_t(cur);
-        const float4 nrx = __ldg(nd + nx), frx = __ldg(nd + fx), nry = __ldg(nd + ny), fry = __ldg(nd + fy), nrz = __ldg(nd + nz), frz = __ldg(nd + fz);
-        lk = __ldg(reinterpret_cast<const int4 *>(nd + 6));
-#define TGB_SLAB(K, OUT) { \
-            float ax = __fmaf_rn(nrx.K, idx, -oodx), bx = __fmaf_rn(frx.K, idx, -oodx); \
-            float ay = __fmaf_rn(nry.K, idy, -oody), by = __fmaf_rn(fry.K, idy, -oody); \
-            float az = __fmaf_rn(nrz.K, idz, -oodz), bz = __fmaf_rn(frz.K, idz, -oodz); \
-            float tmn = fmaxf(fmaxf(fmaxf(ax, ay), az), tnear); float tmx = fminf(fminf(fminf(bx, by), bz), h.t); \
-            OUT = (tmn <= tmx && lk.K != EMPTY) ? tmn : INFINITY; }
-        TGB_SLAB(x, t0) TGB_SLAB(y, t1) TGB_SLAB(z, t2) TGB_SLAB(w, t3)
-#undef TGB_SLAB
-        (void)treelet;
-#endif
-    }
-#if TGB_QNODES
-    // the arithmetic of a visit on a node that is already in registers (the machine can fetch a node one trip ahead)
-    TGB_D void visit_loaded(const DScene &sc, const uint4 c0, const uint4 c1, const uint4 c2, const int4 lk, float &t0, float &t1, float &t2, float &t3) {
+    TGB_D void visit(const DScene &sc, float &t0, float &t1, float &t2, float &t3, int4 &lk) {
+        const uint4 *nd = sc.qnodes + 4*size_t(cur);
+        const uint4 c0 = __ldg(nd), c1 = __ldg(nd + 1), c2 = __ldg(nd + 2); lk = __ldg(reinterpret_cast<const int4 *>(nd + 3));
         const float ax_ = __uint_as_float(c0.w)*idx, ay_ = __uint_as_float(c1.x)*idy, az_ = __uint_as_float(c1.y)*idz;
         const float bx_ = __fmaf_rn(__uint_as_float(c0.x), idx, -oodx) - ax_;
         const float by_ = __fmaf_rn(__uint_as_float(c0.y), idy, -oody) - ay_;
@@ -423,14 +357,9 @@ struct Traversal {
         TGB_SLAB(0, lk.x, t0) TGB_SLAB(1, lk.y, t1) TGB_SLAB(2, lk.z, t2) TGB_SLAB(3, lk.w, t3)
 #undef TGB_SLAB
     }
-#endif
 
-    // Moeller-Trumbore on leaf-order record k; true (and h updated) when it is hit closer than h.t
-    TGB_D bool triangle(const DScene &sc, int k) {
-        const float4 *tr = sc.tri_isect + 3*size_t(k);
-        return triangle_rec(__ldg(tr), __ldg(tr + 1), __ldg(tr + 2), k);
-    }
-    TGB_D bool triangle_rec(const float4 a, const float4 b, const float4 c, int k) {
+    // Moeller-Trumbore on leaf-order record k (a, b, c = its three float4); true (and h updated) when it is hit closer than h.t
+    TGB_D bool triangle(const float4 a, const float4 b, const float4 c, int k) {
         V3 v0 = v3(a.x, a.y, a.z), e1 = v3(a.w, b.x, b.y), e2 = v3(b.z, b.w, c.x), ng = v3(c.y, c.z, c.w);
         V3 C = v0 - o;
         V3 R = cross(d, C);
@@ -460,203 +389,45 @@ struct Traversal {
         }
         return false;
     }
-
-    template <class Y>
-    TGB_D bool run(const DScene &sc, const uint4 *treelet, TravStack &stk, int &sp, Y yield) {
-        while (true) {
-        while (cur >= 0) {
-            float t0, t1, t2, t3; int4 lk;
-            visit(sc, treelet, t0, t1, t2, t3, lk);
-            int l0 = lk.x, l1 = lk.y, l2 = lk.z, l3 = lk.w;
-            TGB_CSWAP(t0, l0, t1, l1) TGB_CSWAP(t2, l2, t3, l3) TGB_CSWAP(t0, l0, t2, l2) TGB_CSWAP(t1, l1, t3, l3) TGB_CSWAP(t1, l1, t2, l2)
-            if (t0 == INFINITY) {
-                if (sp == 0) return true;
-                cur = stk.pop(sp);
-            } else {
-                // sorted, so the children to push are a prefix of (l1, l2, l3); the nearest of them must end up on top
-                const bool p1 = t1 != INFINITY, p2 = t2 != INFINITY, p3 = t3 != INFINITY;
-                if (sp + 3 <= kSmemStack) {
-                    // slot of l3 = sp, of l2 = sp + [p3], of l1 = sp + [p3] + [p2]
-                    const uint32_t a3 = stk.base + uint32_t(sp)*(kTraceBlock*4u);
-                    const uint32_t a2 = a3 + (p3 ? kTraceBlock*4u : 0u), a1 = a2 + (p2 ? kTraceBlock*4u : 0u);
-                    if (p3) TravStack::sts(a3, l3);
-                    if (p2) TravStack::sts(a2, l2);
-                    if (p1) TravStack::sts(a1, l1);
-                    sp += int(p1) + int(p2) + int(p3);
-                } else {
-                    if (p3) stk.push(sp, l3);
-                    if (p2) stk.push(sp, l2);
-                    if (p1) stk.push(sp, l1);
-                }
-                cur = l0;
-            }
-        }
-        int code = ~cur;
-        int first = code >> 3, count = (code & 3) + 1;
-        if ((code & 4) && (!CURVES || first >= sc.analytic_base)) {
-            if (analytic_leaf(sc, first, count)) return true;
-        } else
-        if (CURVES && (code & 4)) {
-            for (int i = 0; i < count; ++i) {
-                int seg = int(__ldg(sc.tri_global + first + i) - sc.n_tris)/kCurvePieces;     // global id of a curve record: n_tris + 4*segment + quarter
-                if (seg == last_seg) continue;
-                last_seg = seg;
-                const float4 *cr = sc.tri_isect + 3*size_t(first + i);
-                float4 q0 = curve_project(o, cf, d, __ldg(cr)), q1 = curve_project(o, cf, d, __ldg(cr + 1)), q2 = curve_project(o, cf, d, __ldg(cr + 2));
-                float ht, hu, hw;
-                if (curve_point_on_spline(q0, q1, q2, tnear, h.t, ht, hu, hw)) {
-                    h.t = ht; h.u = hu; h.v = hw; h.id = first + i;
-                    if (any) return true;
-                }
-            }
-        } else
-        for (int i = 0; i < count; ++i) {
-            if (triangle(sc, first + i) && any) return true;
-        }
-        if (sp == 0) return true;
-            cur = stk.pop(sp);
-            if (yield()) return false;
-        }
-    }
 };
 
-template <bool CURVES>
-TGB_D void bvh_traverse(const DScene &sc, const uint4 *treelet, int *smem_stack, V3 o, V3 d, float tnear, bool any, Hit &h) {
-    Traversal<CURVES> tr; TravStack stk; stk.base = smem_addr(smem_stack + threadIdx.x); int sp = 0;
-    tr.begin(o, d, tnear, any, h);
-    tr.run(sc, treelet, stk, sp, [] { return false; });
-    h = tr.h;
-}
-
-// Persistent form used by the renderer's traversal kernels: a fixed grid of warps pulls rays from a shared counter.  A
-// ray's traversal length is heavy-tailed, so with one ray per lane a warp spends most of its life with a quarter of its
-// lanes alive; here, whenever fewer than kRefillBelow lanes are still walking,
-// the warp pauses at the next leaf boundary and the idle lanes fetch the next rays of the (coherence-sorted) queue.
-#ifndef TGB_REFILL_BELOW
-#define TGB_REFILL_BELOW 20
-#endif
+// Persistent form used by the renderer's traversal kernels: a fixed grid of warps pulls rays from a shared counter, and
+// each warp runs a STATE MACHINE over its lanes' rays.  A ray's traversal length is heavy-tailed, and a segment test is a
+// data-dependent bisection of 1..63 steps: with a per-lane walk the kernel was issue bound with a few of 32 threads active
+// per instruction -- every lane waiting for the warp's longest ray or bisection.  Here each lane is in one of four states and
+// every trip of the loop runs ONE block of code for all the lanes that are in the state most lanes are in:
+//      NODE    one 4-ary node visit                          LEAF   next primitive of the leaf: triangle tests, or the set-up
+//      BISECT  one step of pointOnSpline (box test, split     CYL    intersectHalfCylinder of a depth-5 piece, then pop
+//              or pop)
+// so a lane in a long bisection no longer stalls the others: they go on visiting nodes and starting their own segment tests in
+// the same trips.  A ray's arithmetic and the order of ITS node visits / segment tests are unchanged (parity unaffected).
+// Once enough lanes are idle, the warp pulls the next rays of the (coherence-sorted) queue into them.
 // resident blocks the CURVE instantiations of the traversal kernels are compiled for (4 x 128 threads: up to 128 registers; the
 // state machine keeps a ray's traversal AND bisection state live, and it is issue bound, not latency bound)
 #ifndef TGB_MINB_CURVES
 #define TGB_MINB_CURVES 5
 #endif
-template <bool CURVES, class P>
-TGB_D void machine_traverse_persistent(const DScene &sc, const uint4 *treelet, int *smem_stack, P &pol, uint32_t n, uint32_t *counter);
-// 1 = triangle-only scenes go through the state machine too (measured faster than the while-while form, B200)
-#ifndef TGB_MACHINE_TRIS
-#define TGB_MACHINE_TRIS 1
-#endif
-template <bool CURVES, class P>
-TGB_D void bvh_traverse_persistent(const DScene &sc, const uint4 *treelet, int *smem_stack, P &pol, uint32_t n, uint32_t *counter) {
-    if constexpr (CURVES || TGB_MACHINE_TRIS) { machine_traverse_persistent<CURVES>(sc, treelet, smem_stack, pol, n, counter); return; }
-    const unsigned FULL = 0xffffffffu, lane = threadIdx.x & 31u;
-    Traversal<CURVES> tr; TravStack stk; stk.base = smem_addr(smem_stack + threadIdx.x); int sp = 0;
-    bool active = false, exhausted = false;
-    for (;;) {
-        unsigned need = __ballot_sync(FULL, !active);
-        if (need && !exhausted) {
-            unsigned cnt = unsigned(__popc(need)), leader = unsigned(__ffs(int(need))) - 1u;
-            uint32_t base = 0;
-            if (lane == leader) base = atomicAdd(counter, cnt);
-            base = __shfl_sync(FULL, base, int(leader));
-            exhausted = base + cnt >= n;
-            if (!active) {
-                uint32_t i = base + unsigned(__popc(need & ((1u << lane) - 1u)));
-                V3 o, d; float tnear; Hit h; bool any;
-                if (i < n && pol.fetch(i, o, d, tnear, h, any)) { tr.begin(o, d, tnear, any, h); tr.ignore = pol.ignore(); sp = 0; active = true; }
-            }
-        }
-        if (!__any_sync(FULL, active)) break;
-        if (active) {
-            const bool may_refill = !exhausted;
-            bool done = tr.run(sc, treelet, stk, sp, [=] { return may_refill && __popc(__activemask()) < TGB_REFILL_BELOW; });
-            if (done) { pol.finish(tr.h); active = false; }
-        }
-    }
-}
-
-// Curve scenes: the same persistent loop as a warp-level STATE MACHINE.  A segment test is a data-dependent bisection of 1..63
-// steps and the while-while form above ran it inside the leaf loop of each lane: the kernel was issue bound with a few of
-// 32 threads active per instruction -- every lane waiting for the warp's longest bisection.  Here each lane is in one of four states and every trip of the loop runs ONE block
-// of code for all the lanes that are in the state most lanes are in:
-//      NODE    one 4-ary node visit                          LEAF   next primitive of the leaf: triangle tests, or the set-up
-//      BISECT  one step of pointOnSpline (box test, split     CYL    intersectHalfCylinder of a depth-5 piece, then pop
-//              or pop)
-// so a lane in a long bisection no longer stalls the others: they go on visiting nodes and starting their own segment tests in
-// the same trips.  A ray's arithmetic and the order of ITS node visits / segment tests are unchanged (parity unaffected);
-// idle lanes are refilled from the ray cursor as above.
 // idle lanes a warp tolerates before it pulls new rays
 #ifndef TGB_CURVE_REFILL_IDLE
 #define TGB_CURVE_REFILL_IDLE 8
 #endif
-// rays a warp reserves from the queue cursor per atomicAdd; 0 = exactly the idle lanes of each refill.  Reserving ahead saves
-// atomics but leaves the reserved rays waiting for ONE warp at the end of a launch
-#ifndef TGB_RAY_CHUNK
-#define TGB_RAY_CHUNK 0
-#endif
-// 1 = the machine tests ONE triangle per LEAF trip and loads the next triangle's record a trip ahead (12 more registers)
-#ifndef TGB_TRI_PREFETCH
-#define TGB_TRI_PREFETCH 0
-#endif
-// 1 = the machine fetches a node's 64 bytes when the node becomes current (end of the previous NODE trip, pop, ray start) instead
-// of at the start of its visit: 16 more registers, the fetch overlaps the trips in between
-#ifndef TGB_NODE_PREFETCH
-#define TGB_NODE_PREFETCH 0
-#endif
-// triangle records the machine's LEAF block keeps in flight: 0 = one (load, test, load, ...), 1 = two, 2 = the whole leaf
-#ifndef TGB_LEAF_PAIRS
-#define TGB_LEAF_PAIRS 1
-#endif
 #ifndef TGB_TRI_REFILL_IDLE
 #define TGB_TRI_REFILL_IDLE 16
 #endif
-#ifndef TGB_CM_WN            // scheduling weights of the four blocks (the block with the largest weight x lanes runs)
-#define TGB_CM_WN 4
-#endif
-#ifndef TGB_CM_WL
-#define TGB_CM_WL 4
-#endif
-#ifndef TGB_CM_WB
-#define TGB_CM_WB 4
-#endif
-#ifndef TGB_CM_WC
-#define TGB_CM_WC 4
-#endif
 enum : int { CM_IDLE = 0, CM_NODE = 1, CM_LEAF = 2, CM_BISECT = 3, CM_CYL = 4 };
 template <bool CURVES, class P>
-TGB_D void machine_traverse_persistent(const DScene &sc, const uint4 *treelet, int *smem_stack, P &pol, uint32_t n, uint32_t *counter) {
+TGB_D void bvh_traverse_persistent(const DScene &sc, int *smem_stack, P &pol, uint32_t n, uint32_t *counter) {
     const unsigned FULL = 0xffffffffu, lane = threadIdx.x & 31u;
-    constexpr int kW[4] = {TGB_CM_WN, TGB_CM_WL, TGB_CM_WB, TGB_CM_WC};
     Traversal<CURVES> tr; TravStack stk; stk.base = smem_addr(smem_stack + threadIdx.x); int sp = 0;
     int mode = CM_IDLE; bool exhausted = false;
-    uint32_t chunk_next = 0, chunk_end = 0; (void)chunk_next; (void)chunk_end;
     int li = 0, prim = 0; bool seg_hit = false;                                        // leaf cursor, BVH primitive under test
     float4 q0 = {}, q1 = {}, q2 = {}, c0 = {}, c1 = {};                                 // the segment's quadratic, the current piece's end points
     float tFlatX = 0.0f, tFlatY = 0.0f, xFlat = 0.0f, yFlat = 0.0f, pMin = 0.0f, pMax = 1.0f;
     uint32_t bidx = 0, pending = 0; int depth = 0;                                      // piece = [bidx, bidx + 1]/2^depth; pending siblings by depth
     auto finish_ray = [&]() { pol.finish(tr.h); mode = CM_IDLE; };
-#if TGB_TRI_PREFETCH
-    float4 ra = {}, rb = {}, rc = {};                                                   // the triangle record the next LEAF trip tests
-    auto prefetch_tri = [&](int link, int i) {
-        const int code = ~link;
-        if (!(code & 4)) { const float4 *t = sc.tri_isect + 3*size_t((code >> 3) + i); ra = __ldg(t); rb = __ldg(t + 1); rc = __ldg(t + 2); }
-    };
-#else
-    auto prefetch_tri = [&](int, int) {};
-#endif
-#if TGB_NODE_PREFETCH && TGB_QNODES
-    uint4 n0 = {}, n1 = {}, n2 = {}; int4 nl = {};
-    auto prefetch_node = [&](int node) {
-        const uint4 *nd = sc.qnodes + 4*size_t(node);
-        n0 = __ldg(nd); n1 = __ldg(nd + 1); n2 = __ldg(nd + 2); nl = __ldg(reinterpret_cast<const int4 *>(nd + 3));
-    };
-#else
-    auto prefetch_node = [&](int) {};
-#endif
     auto pop_node = [&]() {                                                             // leave a leaf: next stack entry or done
         if (sp == 0) { finish_ray(); return; }
         tr.cur = stk.pop(sp); li = 0; mode = tr.cur >= 0 ? CM_NODE : CM_LEAF;
-        if (tr.cur < 0) prefetch_tri(tr.cur, 0); else prefetch_node(tr.cur);
     };
     // box test of pointOnSpline's loop head for the piece (a, b) = the curve on [ta, tb]
     auto piece_box = [&](const float4 &a, const float4 &b, float ta, float tb) {
@@ -688,36 +459,22 @@ TGB_D void machine_traverse_persistent(const DScene &sc, const uint4 *treelet, i
     for (;;) {
         const unsigned idle = __ballot_sync(FULL, mode == CM_IDLE);
         if (!exhausted && __popc(idle) >= (CURVES ? TGB_CURVE_REFILL_IDLE : TGB_TRI_REFILL_IDLE)) {
-#if TGB_RAY_CHUNK
-            // the warp owns rays [chunk_next, chunk_end) of the queue: one atomicAdd per TGB_RAY_CHUNK rays instead of one per refill
-            if (chunk_next == chunk_end) {
-                uint32_t b = 0;
-                if (lane == 0) b = atomicAdd(counter, uint32_t(TGB_RAY_CHUNK));
-                b = __shfl_sync(FULL, b, 0);
-                if (b >= n) { exhausted = true; continue; }
-                chunk_next = b; chunk_end = min(b + uint32_t(TGB_RAY_CHUNK), n);
-            }
-            const uint32_t rank = unsigned(__popc(idle & ((1u << lane) - 1u)));
-            const uint32_t cnt = min(uint32_t(__popc(idle)), chunk_end - chunk_next);
-            const uint32_t first_ray = chunk_next;
-            chunk_next += cnt;
-#else
             const uint32_t cnt = unsigned(__popc(idle)), leader = unsigned(__ffs(int(idle))) - 1u;
             const uint32_t rank = unsigned(__popc(idle & ((1u << lane) - 1u)));
             uint32_t first_ray = 0;
             if (lane == leader) first_ray = atomicAdd(counter, cnt);
             first_ray = __shfl_sync(FULL, first_ray, int(leader));
             exhausted = first_ray + cnt >= n;
-#endif
             if (mode == CM_IDLE && rank < cnt && first_ray + rank < n) {
                 V3 o, d; float tnear; Hit h; bool any;
-                if (pol.fetch(first_ray + rank, o, d, tnear, h, any)) { tr.begin(o, d, tnear, any, h); tr.ignore = pol.ignore(); sp = 0; mode = CM_NODE; prefetch_node(0); }
+                if (pol.fetch(first_ray + rank, o, d, tnear, h, any)) { tr.begin(o, d, tnear, any, h); tr.ignore = pol.ignore(); sp = 0; mode = CM_NODE; }
             }
             continue;
         }
         if (idle == FULL) break;                                                        // (only reached once the cursor is exhausted)
-        const int sN = kW[0]*__popc(__ballot_sync(FULL, mode == CM_NODE)), sL = kW[1]*__popc(__ballot_sync(FULL, mode == CM_LEAF));
-        const int sB = CURVES ? kW[2]*__popc(__ballot_sync(FULL, mode == CM_BISECT)) : -1, sC = CURVES ? kW[3]*__popc(__ballot_sync(FULL, mode == CM_CYL)) : -1;
+        // the block most lanes are in runs (ties: BISECT, CYL, NODE, LEAF); triangle scenes have no curve states
+        const int sN = __popc(__ballot_sync(FULL, mode == CM_NODE)), sL = __popc(__ballot_sync(FULL, mode == CM_LEAF));
+        const int sB = CURVES ? __popc(__ballot_sync(FULL, mode == CM_BISECT)) : -1, sC = CURVES ? __popc(__ballot_sync(FULL, mode == CM_CYL)) : -1;
         const int best = max(max(sN, sL), max(sB, sC));
         if (CURVES && sB == best) {
             // BISECT: split a piece that passed its box test (depth < 5) and test BOTH halves: the near half is entered if it
@@ -757,11 +514,7 @@ TGB_D void machine_traverse_persistent(const DScene &sc, const uint4 *treelet, i
         } else if (sN == best) {
             if (mode == CM_NODE) {
                 float t0, t1, t2, t3; int4 lk;
-#if TGB_NODE_PREFETCH && TGB_QNODES
-                lk = nl; tr.visit_loaded(sc, n0, n1, n2, nl, t0, t1, t2, t3);
-#else
-                tr.visit(sc, treelet, t0, t1, t2, t3, lk);
-#endif
+                tr.visit(sc, t0, t1, t2, t3, lk);
                 int l0 = lk.x, l1 = lk.y, l2 = lk.z, l3 = lk.w;
                 TGB_CSWAP(t0, l0, t1, l1) TGB_CSWAP(t2, l2, t3, l3) TGB_CSWAP(t0, l0, t2, l2) TGB_CSWAP(t1, l1, t3, l3) TGB_CSWAP(t1, l1, t2, l2)
                 if (t0 == INFINITY) pop_node();
@@ -781,7 +534,7 @@ TGB_D void machine_traverse_persistent(const DScene &sc, const uint4 *treelet, i
                         if (p1) stk.push(sp, l1);
                     }
                     tr.cur = l0;
-                    if (l0 < 0) { mode = CM_LEAF; li = 0; prefetch_tri(l0, 0); } else prefetch_node(l0);
+                    if (l0 < 0) { mode = CM_LEAF; li = 0; }
                 }
             }
         } else {
@@ -811,45 +564,17 @@ TGB_D void machine_traverse_persistent(const DScene &sc, const uint4 *treelet, i
                     }
                     if (!started) pop_node();
                 } else {
-#if TGB_TRI_PREFETCH
-                    const bool hit_any = tr.triangle_rec(ra, rb, rc, first + li) && tr.any;
-                    ++li;
-                    if (hit_any) finish_ray();
-                    else if (li < count) prefetch_tri(tr.cur, li);
-                    else pop_node();
-#else
-                    bool hit_any = false;
-#if TGB_LEAF_PAIRS == 2
-                    // the whole leaf (<= 4 records) in flight before the first test
-                    {
-                        const float4 *t = sc.tri_isect + 3*size_t(first);
-                        const int k1 = count > 1 ? 3 : 0, k2 = count > 2 ? 6 : 0, k3 = count > 3 ? 9 : 0;
-                        const float4 a0 = __ldg(t), b0 = __ldg(t + 1), c0 = __ldg(t + 2);
-                        const float4 a1 = __ldg(t + k1), b1 = __ldg(t + k1 + 1), c1 = __ldg(t + k1 + 2);
-                        const float4 a2 = __ldg(t + k2), b2 = __ldg(t + k2 + 1), c2 = __ldg(t + k2 + 2);
-                        const float4 a3 = __ldg(t + k3), b3 = __ldg(t + k3 + 1), c3 = __ldg(t + k3 + 2);
-                        hit_any = tr.triangle_rec(a0, b0, c0, first) && tr.any;
-                        if (count > 1 && !hit_any) hit_any = tr.triangle_rec(a1, b1, c1, first + 1) && tr.any;
-                        if (count > 2 && !hit_any) hit_any = tr.triangle_rec(a2, b2, c2, first + 2) && tr.any;
-                        if (count > 3 && !hit_any) hit_any = tr.triangle_rec(a3, b3, c3, first + 3) && tr.any;
-                    }
-#elif TGB_LEAF_PAIRS
                     // two records in flight: the second triangle's loads are issued before the first is tested
+                    bool hit_any = false;
                     for (int i = 0; i < count && !hit_any; i += 2) {
                         const float4 *t = sc.tri_isect + 3*size_t(first + i);
                         const bool two = i + 1 < count;
                         const float4 a0 = __ldg(t), b0 = __ldg(t + 1), c0 = __ldg(t + 2);
                         const float4 a1 = __ldg(t + (two ? 3 : 0)), b1 = __ldg(t + (two ? 4 : 1)), c1 = __ldg(t + (two ? 5 : 2));
-                        hit_any = tr.triangle_rec(a0, b0, c0, first + i) && tr.any;
-                        if (two && !hit_any) hit_any = tr.triangle_rec(a1, b1, c1, first + i + 1) && tr.any;
+                        hit_any = tr.triangle(a0, b0, c0, first + i) && tr.any;
+                        if (two && !hit_any) hit_any = tr.triangle(a1, b1, c1, first + i + 1) && tr.any;
                     }
-#else
-                    for (int i = 0; i < count; ++i) {
-                        if (tr.triangle(sc, first + i) && tr.any) { hit_any = true; break; }
-                    }
-#endif
                     if (hit_any) finish_ray(); else pop_node();
-#endif
                 }
             }
         }
@@ -884,17 +609,6 @@ TGB_D bool mesh_cut_hit(const DScene &sc, V3 o, V3 d, float tnear, float tfar) {
         }
     }
     return hit;
-}
-
-// One ray per thread (parity hook): a policy object supplies the ray and takes the hit.
-template <bool CURVES, class P>
-TGB_D void bvh_traverse_multi(const DScene &sc, int *smem_stack, P &pol, uint32_t n) {
-    uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    V3 o, d; float tnear; Hit h; bool any;
-    if (!pol.fetch(i, o, d, tnear, h, any)) return;
-    bvh_traverse<CURVES>(sc, nullptr, smem_stack, o, d, tnear, any, h);
-    pol.finish(h);
 }
 
 // Fill a Surface from a hit: Primitive::intersectionInfo for mesh/quad/cube
@@ -1149,17 +863,15 @@ struct PathRayPolicy {
 };
 template <bool CURVES>
 __global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_trace(DScene sc, PathBuf pb, const uint32_t *order, Ctl *ctl) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const uint4 *treelet = stage_treelet(sc, smem_raw);
-    int *smem_stack = reinterpret_cast<int *>(smem_raw + size_t(sc.n_treelet)*64);
+    __shared__ int smem_stack[kSmemStack*kTraceBlock];
     PathRayPolicy pol; pol.T0 = pb.T0; pol.T1 = pb.T1; pol.T2 = pb.T2; pol.order = order; pol.n_sorted = ctl->n_sorted; pol.n_surv = ctl->n_surv; pol.n_all = ctl->n; pol.s = 0;
     // rays to pull: the sorted survivors + the new camera paths
     const uint32_t n = ctl->n_sorted + ctl->n_new;
-    bvh_traverse_persistent<CURVES>(sc, treelet, smem_stack, pol, n, &ctl->cursor_trace);
+    bvh_traverse_persistent<CURVES>(sc, smem_stack, pol, n, &ctl->cursor_trace);
 }
 
 // Parity hook (tgb200_trace_closest): rays in AoS tgb_ray, hits out as tgb_hit, through the same analytic pass and
-// the same BVH traversal code as the renderer (global-memory nodes only).
+// the same persistent BVH traversal as the renderer.
 // Rays the analytic pass settled through the BVH's top-level cut are not in `list` (k_hook_analytic).
 struct HookPolicy {
     const tgb_ray *rays; Hit *out; const uint32_t *list, *count; uint32_t i;
@@ -1185,34 +897,11 @@ __global__ void __launch_bounds__(256) k_hook_analytic(DScene sc, const tgb_ray 
     if (!cut || mesh_cut_hit(sc, o, d, rays[i].tmin, h.t)) list[atomicAdd(count, 1u)] = i;
 }
 template <bool CURVES>
-__global__ void __launch_bounds__(kTraceBlock) k_hook_bvh(DScene sc, const tgb_ray *rays, Hit *out, const uint32_t *list,
-                                                         const uint32_t *count, uint32_t n) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    HookPolicy pol; pol.rays = rays; pol.out = out; pol.list = list; pol.count = count; pol.i = 0;
-    bvh_traverse_multi<CURVES>(sc, reinterpret_cast<int *>(smem_raw), pol, n);
-}
-// The same queries through the renderer's PERSISTENT kernel body (treelet staged in shared memory, lane refill): the
-// second half of the hit-id parity check, so the staged copy of the top nodes is pinned as well.
-struct HookPersistPolicy {
-    const tgb_ray *rays; Hit *out; const uint32_t *list, *count; uint32_t i;
-    TGB_D bool fetch(uint32_t idx, V3 &o, V3 &d, float &tnear, Hit &h, bool &any) {
-        if (idx >= *count) return false;
-        i = list[idx];
-        o = v3(rays[i].o[0], rays[i].o[1], rays[i].o[2]); d = v3(rays[i].d[0], rays[i].d[1], rays[i].d[2]); tnear = rays[i].tmin;
-        h = out[i]; any = false;
-        return true;
-    }
-    TGB_D void finish(const Hit &h) { out[i] = h; }
-    TGB_D int ignore() const { return -1; }
-};
-template <bool CURVES>
 __global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_hook_persist(DScene sc, const tgb_ray *rays, Hit *out, const uint32_t *list,
                                                                                           const uint32_t *count, uint32_t n, uint32_t *counter) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const uint4 *treelet = stage_treelet(sc, smem_raw);
-    int *smem_stack = reinterpret_cast<int *>(smem_raw + size_t(sc.n_treelet)*64);
-    HookPersistPolicy pol; pol.rays = rays; pol.out = out; pol.list = list; pol.count = count; pol.i = 0;
-    bvh_traverse_persistent<CURVES>(sc, treelet, smem_stack, pol, n, counter);
+    __shared__ int smem_stack[kSmemStack*kTraceBlock];
+    HookPolicy pol; pol.rays = rays; pol.out = out; pol.list = list; pol.count = count; pol.i = 0;
+    bvh_traverse_persistent<CURVES>(sc, smem_stack, pol, n, counter);
 }
 __global__ void __launch_bounds__(256) k_hook_finish(DScene sc, const tgb_ray *rays, const Hit *in, tgb_hit *hits, uint32_t n) {
     uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
@@ -1591,11 +1280,9 @@ struct ShadowPolicy {
 };
 template <bool CURVES>
 __global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_shadow_bvh(DScene sc, Scratch sr, const uint32_t *squeue, Ctl *ctl, Counters *ctr) {
-    extern __shared__ __align__(128) unsigned char smem_raw[];
-    const uint4 *treelet = stage_treelet(sc, smem_raw);
-    int *smem_stack = reinterpret_cast<int *>(smem_raw + size_t(sc.n_treelet)*64);
+    __shared__ int smem_stack[kSmemStack*kTraceBlock];
     ShadowPolicy<CURVES> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue; pol.hits = &ctr->shadow_hits;
-    bvh_traverse_persistent<CURVES>(sc, treelet, smem_stack, pol, ctl->shadow_count2, &ctl->cursor_shadow);
+    bvh_traverse_persistent<CURVES>(sc, smem_stack, pol, ctl->shadow_count2, &ctl->cursor_shadow);
 }
 
 // Fold this bounce's direct light + surface emission into the path (order as in handleSurface:537-543), apply the
