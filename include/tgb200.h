@@ -279,6 +279,13 @@ int  tgb200_hair_selftest(float roughness, float scale_angle_deg, const float *s
  * force over all triangles, bit for bit.  *mismatches = rays that differ (must be 0).                                   */
 int  tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays,
                           uint32_t *mismatches, uint32_t *n_nodes, uint64_t *node_visits);
+/* Host-only count of the any-hit shadow walk (no GPU): builds n triangles' tree as tgb200_create does, then walks n_queries
+ * occlusion queries (8 floats each: o, d, tnear, t_light) both as a sorted walk from the root and as the unsorted walk from the
+ * top-level cut boxes the segment enters.  out = 10 uint32 per query: cut mask, deepest stack of the cut walk, then per walk
+ * (root, cut): occluded, node visits, leaf trips, triangle tests.  *stack_need = the traversal stack bound tgb200_create checks;
+ * TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the traversal's own stack).                                           */
+int  tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *camera_pos, const float *queries, uint32_t n_queries,
+                              uint32_t stack_size, uint32_t *stack_need, uint32_t *out);
 /* Test hooks: each launches one kernel on the context's stream that calls the device functions the shading kernel calls, on
  * host arrays in and out.  A NULL context returns TGB_ERR_INVALID.
  * tgb200_bsdf_probe: Bsdf::eval(event, adjoint=false) rgb + Bsdf::pdf of bsdf `bsdf` for n (wi, wo) pairs in the local frame

@@ -107,7 +107,7 @@ class SampleRecord(C.Structure):
 EXPORTS = [
     "tgb200_create", "tgb200_render_tiles", "tgb200_render_resident", "tgb200_clear_framebuffer",
     "tgb200_read_framebuffer", "tgb200_write_framebuffer", "tgb200_generate_work", "tgb200_render_adaptive", "tgb200_framebuffer_device_ptr", "tgb200_trace_closest", "tgb200_shard_tiles", "tgb200_pack_tiles", "tgb200_unpack_tiles",
-    "tgb200_get_stats", "tgb200_set_profiling", "tgb200_set_stream", "tgb200_scene_info", "tgb200_reset_stats", "tgb200_bvh_selftest", "tgb200_hair_selftest", "tgb200_qbvh_selftest", "tgb200_bsdf_probe", "tgb200_bsdf_sample_probe", "tgb200_light_probe",
+    "tgb200_get_stats", "tgb200_set_profiling", "tgb200_set_stream", "tgb200_scene_info", "tgb200_reset_stats", "tgb200_bvh_selftest", "tgb200_hair_selftest", "tgb200_qbvh_selftest", "tgb200_shadow_walk_count", "tgb200_bsdf_probe", "tgb200_bsdf_sample_probe", "tgb200_light_probe",
     "tgb200_choose_light_probe", "tgb200_shadow_probe", "tgb200_abort", "tgb200_clear_abort", "tgb200_destroy", "tgb200_last_error",
     "tgb200_abi_version",
 ]

@@ -198,6 +198,39 @@ static void build_from_boxes(std::vector<Box> &tb, std::vector<float> &cent, uin
     }
 }
 
+std::vector<CutBox> top_level_cut(const Bvh4 &bvh, size_t max_cut) {
+    std::vector<CutBox> cut;
+    if (bvh.nodes.empty()) return cut;
+    auto child = [&](const Node4 &nd, int k) { CutBox b; for (int a = 0; a < 3; ++a) { b.lo[a] = nd.f[8*a + k]; b.hi[a] = nd.f[8*a + 4 + k]; } b.link = nd.link[k]; return b; };
+    auto area = [](const CutBox &b) { float e[3] = {b.hi[0] - b.lo[0], b.hi[1] - b.lo[1], b.hi[2] - b.lo[2]}; return e[0]*e[1] + e[1]*e[2] + e[2]*e[0]; };
+    for (int k = 0; k < 4; ++k) if (bvh.nodes[0].link[k] != kEmptyLink) cut.push_back(child(bvh.nodes[0], k));
+    while (true) {
+        int best = -1;
+        for (size_t i = 0; i < cut.size(); ++i) if (cut[i].link >= 0 && (best < 0 || area(cut[i]) > area(cut[size_t(best)]))) best = int(i);
+        if (best < 0) break;
+        const Node4 &nd = bvh.nodes[size_t(cut[size_t(best)].link)];
+        int kids = 0; for (int k = 0; k < 4; ++k) kids += nd.link[k] != kEmptyLink;
+        if (cut.size() - 1 + size_t(kids) > max_cut) break;
+        cut.erase(cut.begin() + best);
+        for (int k = 0; k < 4; ++k) if (nd.link[k] != kEmptyLink) cut.push_back(child(nd, k));
+    }
+    return cut;
+}
+
+uint32_t traversal_stack_need(const Bvh4 &bvh, const std::vector<CutBox> &cut) {
+    // inner nodes on the longest path down from each node (0 for a leaf)
+    std::vector<uint32_t> levels(bvh.nodes.size(), 0);
+    for (size_t i = bvh.nodes.size(); i-- > 0;) {          // children follow their parent in Node4 order (build_from_boxes)
+        uint32_t l = 0;
+        for (int k = 0; k < 4; ++k) if (bvh.nodes[i].link[k] >= 0) l = std::max(l, levels[size_t(bvh.nodes[i].link[k])]);
+        levels[i] = l + 1;
+    }
+    uint32_t below = 0;
+    for (const CutBox &b : cut) if (b.link >= 0) below = std::max(below, levels[size_t(b.link)]);
+    const uint32_t from_cut = cut.empty() ? 0u : uint32_t(cut.size()) - 1u + 3u*below;
+    return std::max(3u*bvh.max_depth + 2u, from_cut);
+}
+
 // ---- quantised layout -------------------------------------------------------------------------------------------
 void quantize_bvh4(const Bvh4 &in, QBvh4 &out, int32_t empty_link) {
     out.nodes.clear(); out.old_index.clear();

@@ -65,6 +65,16 @@ void quantize_bvh4(const Bvh4 &in, QBvh4 &out, int32_t empty_link = kEmptyLink);
 // four children for the ray (o, 1/d), INFINITY where the slab test fails.
 void qnode_slab_host(const QNode4 &nd, const float o[3], const float inv_d[3], float tnear, float tfar, float t_out[4]);
 
+// Top-level cut of a 4-ary tree: start from the root's children and keep replacing the inner child with the largest surface area
+// by its children while there are at most max_cut (<= 16) boxes.  Together the boxes cover every primitive; `link` is the
+// Node4 index (or leaf code) below each.
+struct CutBox { float lo[3], hi[3]; int32_t link; };
+std::vector<CutBox> top_level_cut(const Bvh4 &bvh, size_t max_cut);
+// Traversal stack entries a walk may need: a walk from the root pushes at most 3 per inner node on its path (3*max_depth + 2,
+// kept from before the cut), an any-hit walk starts with the entered cut boxes less the one it enters (< cut.size()) and pushes
+// at most 3 per inner node below a cut box.
+uint32_t traversal_stack_need(const Bvh4 &bvh, const std::vector<CutBox> &cut);
+
 // A primitive given by its bounds and the point the SAH binning sorts it by (curve segments).
 struct BuildBox { float lo[3], hi[3], centroid[3]; };
 

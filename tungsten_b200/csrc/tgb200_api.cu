@@ -60,6 +60,8 @@ struct tgb_ctx {
     PathBuf pb[2]{};                // persistent path state, double buffered (k_accum compacts from one into the other)
     Scratch sr{};                   // per-bounce scratch records + per-step results
     uint32_t *order = nullptr, *squeue = nullptr, *squeue2 = nullptr;   // ray-coherence visiting order of k_trace; shadow-query queues (emitted / left after the analytic pass)
+    uint32_t *squeue_cl = nullptr;  // ... the closest-hit (mesh-light) queries left after the analytic pass
+    bool mesh_lights = false;       // a mesh is a light: closest-hit shadow queries exist, k_shadow_bvh<., false> runs
     uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels
     bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
@@ -610,30 +612,17 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         sc.bin_lo = v3(lo[0], lo[1], lo[2]);
         sc.bin_inv = v3(16.0f/(hi[0] - lo[0]), 16.0f/(hi[1] - lo[1]), 16.0f/(hi[2] - lo[2]));
     }
-    sc.n_cut = 0;
-    if (!bvh.nodes.empty()) {
-        // top-level cut: start from the root's children, keep splitting the inner child with the largest surface area
-        struct CutBox { float lo[3], hi[3]; int32_t link; };
-        auto child = [&](const Node4 &nd, int k) { CutBox b; for (int a = 0; a < 3; ++a) { b.lo[a] = nd.f[8*a + k]; b.hi[a] = nd.f[8*a + 4 + k]; } b.link = nd.link[k]; return b; };
-        auto area = [](const CutBox &b) { float e[3] = {b.hi[0] - b.lo[0], b.hi[1] - b.lo[1], b.hi[2] - b.lo[2]}; return e[0]*e[1] + e[1]*e[2] + e[2]*e[0]; };
-        std::vector<CutBox> cut;
-        size_t max_cut = 16;                     // TGB_CUT_BOXES: fewer boxes = cheaper pre-test in k_accum / k_shadow_prep, looser cut
-        if (const char *e = getenv("TGB_CUT_BOXES")) max_cut = size_t(std::min(16, std::max(4, atoi(e))));
-        for (int k = 0; k < 4; ++k) if (bvh.nodes[0].link[k] != kEmptyLink) cut.push_back(child(bvh.nodes[0], k));
-        while (true) {
-            int best = -1;
-            for (size_t i = 0; i < cut.size(); ++i) if (cut[i].link >= 0 && (best < 0 || area(cut[i]) > area(cut[size_t(best)]))) best = int(i);
-            if (best < 0) break;
-            const Node4 &nd = bvh.nodes[size_t(cut[size_t(best)].link)];
-            int kids = 0; for (int k = 0; k < 4; ++k) kids += nd.link[k] != kEmptyLink;
-            if (cut.size() - 1 + size_t(kids) > max_cut) break;
-            cut.erase(cut.begin() + best);
-            for (int k = 0; k < 4; ++k) if (nd.link[k] != kEmptyLink) cut.push_back(child(nd, k));
-        }
-        sc.n_cut = int(cut.size());
-        for (int i = 0; i < sc.n_cut; ++i) for (int a = 0; a < 3; ++a) { sc.cut[2*a][i] = cut[size_t(i)].lo[a]; sc.cut[2*a + 1][i] = cut[size_t(i)].hi[a]; }
+    size_t max_cut = 16;                         // TGB_CUT_BOXES: fewer boxes = cheaper pre-test in k_accum / k_shadow_prep, looser cut
+    if (const char *e = getenv("TGB_CUT_BOXES")) max_cut = size_t(std::min(16, std::max(4, atoi(e))));
+    const std::vector<CutBox> cut = top_level_cut(bvh, max_cut);
+    sc.n_cut = int(cut.size());
+    for (int i = 0; i < sc.n_cut; ++i) for (int a = 0; a < 3; ++a) { sc.cut[2*a][i] = cut[size_t(i)].lo[a]; sc.cut[2*a + 1][i] = cut[size_t(i)].hi[a]; }
+    {
+        const char *e = getenv("TGB_SHADOW_CUT_ENTRY");
+        sc.cut_entry = (e && e[0] == '0') ? 0 : 1;
     }
-    if (3*bvh.max_depth + 2 > uint32_t(kStackSize)) return fail(c, TGB_ERR_UNSUPPORTED, "BVH depth %u exceeds the traversal stack", bvh.max_depth);
+    const uint32_t stack_need = traversal_stack_need(bvh, cut);
+    if (stack_need > uint32_t(kStackSize)) return fail(c, TGB_ERR_UNSUPPORTED, "BVH depth %u (%u stack entries) exceeds the traversal stack", bvh.max_depth, stack_need);
     c->bvh_depth = bvh.max_depth; c->n_tris = uint32_t(btris.size()); c->bvh_sah = bvh.sah_cost;
     std::vector<float4> tri_isect(3*(btris.size() + cboxes.size() + 1), make_float4(0.0f, 0.0f, 0.0f, 0.0f));   // + one all-zero record: the target of empty child slots
     for (size_t k = btris.size(); k < bvh.order.size(); ++k) {      // curve records: the segment's three nodes + which quarter, leaf order
@@ -653,6 +642,11 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
     // empty child slots link to a one-triangle leaf holding the all-zero record behind the last primitive (den == 0: rejected)
     const int32_t empty_link = ~int32_t(uint32_t(btris.size() + cboxes.size()) << 3);
     QBvh4 qb; quantize_bvh4(bvh, qb, empty_link);
+    {
+        std::vector<int32_t> new_index(qb.old_index.size());
+        for (size_t i = 0; i < qb.old_index.size(); ++i) new_index[size_t(qb.old_index[i])] = int32_t(i);
+        for (int i = 0; i < sc.n_cut; ++i) sc.cut_link[i] = cut[size_t(i)].link >= 0 ? new_index[size_t(cut[size_t(i)].link)] : cut[size_t(i)].link;
+    }
     c->geom_bytes = qb.nodes.size()*sizeof(QNode4) + tri_isect.size()*16 + tri_shade.size()*16 + bvh.order.size()*8;
 
     int rc;
@@ -662,6 +656,7 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
     c->prim_types.resize(prims.size());
     for (size_t i = 0; i < prims.size(); ++i) c->prim_types[i] = prims[i].type;
     c->light_ids = lights;
+    for (int li : lights) c->mesh_lights = c->mesh_lights || prims[size_t(li)].type == TGB_PRIM_MESH;
     std::vector<uint32_t> slots(d->bsdf_slots, d->bsdf_slots + d->n_bsdf_slots);
     if ((rc = dev_upload(c, &sc.slots, slots))) return rc;
     if ((rc = dev_upload(c, &sc.tex, dtex))) return rc;
@@ -720,8 +715,10 @@ int alloc_wavefront(tgb_ctx *c, uint32_t capacity) {
         if ((rc = dev_alloc(c, p, capacity))) return rc;
     if ((rc = dev_alloc(c, &c->sr.vis, size_t(capacity)*2))) return rc;
     if ((rc = dev_alloc(c, &c->sr.SH, size_t(capacity)*2))) return rc;
+    if ((rc = dev_alloc(c, &c->sr.cut_mask, size_t(capacity)*2))) return rc;
     if ((rc = dev_alloc(c, &c->squeue, size_t(capacity)*2))) return rc;
     if ((rc = dev_alloc(c, &c->squeue2, size_t(capacity)*2))) return rc;
+    if ((rc = dev_alloc(c, &c->squeue_cl, size_t(capacity)*2))) return rc;
     if ((rc = dev_alloc(c, &c->order, capacity))) return rc;
     if ((rc = dev_alloc(c, &c->bin_keys, capacity))) return rc;
     if ((rc = dev_alloc(c, &c->bin_hist, size_t(kBins) + 4))) return rc;
@@ -799,6 +796,18 @@ int ensure_results(tgb_ctx *c, size_t n_paths) {
     return TGB_OK;
 }
 
+// k_shadow_bvh over the any-hit queue and (scenes with mesh lights) the closest-hit queue
+void launch_shadow_bvh(tgb_ctx *c, uint32_t grid) {
+    const DScene &sc = c->sc; cudaStream_t st = c->stream;
+    if (c->has_curves) {
+        if (c->mesh_lights) k_shadow_bvh<true, true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
+        else k_shadow_bvh<true, false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
+    } else {
+        if (c->mesh_lights) k_shadow_bvh<false, true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
+        else k_shadow_bvh<false, false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
+    }
+}
+
 // One iteration's kernels.  `bound` >= the iteration's ctl.n: grids are upper bounds, the kernels read the real sizes from
 // the device-resident control block.
 void enqueue_iteration(tgb_ctx *c, const BatchInfo &bi, int cur, uint32_t bound, int slot, uint64_t &launches) {
@@ -827,16 +836,11 @@ void enqueue_iteration(tgb_ctx *c, const BatchInfo &bi, int cur, uint32_t bound,
     }
     launches++;
     if (prof) cudaEventRecord(c->ev_k[slot][3], st);
-    if (curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->ctr);
-    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->ctr);
+    if (curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
+    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
     launches++;
     if (prof) cudaEventRecord(c->ev_k[slot][4], st);
-    if (has_bvh) {
-        uint32_t grid = std::min(blocks(2*bound, kTraceBlock), c->persist_blocks);
-        if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
-        else k_shadow_bvh<false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
-        launches++;
-    }
+    if (has_bvh) { launch_shadow_bvh(c, std::min(blocks(2*bound, kTraceBlock), c->persist_blocks)); launches++; }
     if (prof) cudaEventRecord(c->ev_k[slot][5], st);
     k_accum<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, nxt, c->sr, bi, c->ctl, c->bin_keys, c->bin_hist); launches++;
     if (prof) cudaEventRecord(c->ev_k[slot][6], st);
@@ -1168,8 +1172,8 @@ static int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
             auto prep = [&](auto kern, int *nb) {
                 if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(nb, kern, kTraceBlock, 0);
             };
-            if (c->has_curves) { prep(k_trace<true>, &b1); prep(k_shadow_bvh<true>, &b2); }
-            else { prep(k_trace<false>, &b1); prep(k_shadow_bvh<false>, &b2); }
+            if (c->has_curves) { prep(k_trace<true>, &b1); prep(c->mesh_lights ? k_shadow_bvh<true, true> : k_shadow_bvh<true, false>, &b2); }
+            else { prep(k_trace<false>, &b1); prep(c->mesh_lights ? k_shadow_bvh<false, true> : k_shadow_bvh<false, false>, &b2); }
             if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
             const char *mult = getenv("TGB_PERSIST_MULT");
             c->persist_blocks = uint32_t(sms*std::min(b1, b2))*uint32_t(mult ? std::max(1, atoi(mult)) : 2);
@@ -1619,6 +1623,24 @@ int tgb200_generate_work(tgb_sample_record *records, uint32_t res_x, uint32_t re
     return 1;
 }
 
+namespace {
+// Traversal::triangle on the host: best = t when the triangle is hit in (tnear, best)
+bool host_triangle(const BuildTri &tri, const V3 &o, const V3 &d, float tnear, float &best) {
+    V3 v0 = f3(tri.v0), v1 = f3(tri.v1), v2 = f3(tri.v2);
+    V3 e1 = v0 - v1, e2 = v2 - v0, ng = cross(e1, e2);
+    V3 C = v0 - o, R = cross(d, C);
+    auto edot = [](V3 a, V3 b) { return a.x*b.x + (a.y*b.y + a.z*b.z); };
+    float den = edot(ng, d), absDen = std::fabs(den);
+    auto xs = [&](float a) { return den < 0.0f || (den == 0.0f && std::signbit(den)) ? -a : a; };
+    float U = xs(edot(R, e2)), V = xs(edot(R, e1));
+    if (!(den != 0.0f && U >= 0.0f && V >= 0.0f && U + V <= absDen)) return false;
+    float T = xs(edot(ng, C));
+    if (!(T > absDen*tnear && T < absDen*best)) return false;
+    best = T/absDen;
+    return true;
+}
+}  // namespace
+
 // Host-only check of the quantised device BVH (no GPU needed): builds the 4-ary SAH tree over n triangles exactly as
 // tgb200_create does (same padding), quantises it (QNode4), and walks it on the HOST with the kernels' node
 // arithmetic (qnode_slab_host mirrors Traversal::visit) and their triangle test for every ray (8 floats: o, d, tmin, tmax).
@@ -1644,19 +1666,7 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
             else if (l < 0 || size_t(l) >= qb.nodes.size() || qb.old_index[size_t(l)] != src.link[k]) return TGB_ERR_INVALID;
         }
     }
-    auto tri_test = [&](uint32_t t, const V3 &o, const V3 &d, float tnear, float &best) {   // Traversal::triangle
-        V3 v0 = f3(tris[t].v0), v1 = f3(tris[t].v1), v2 = f3(tris[t].v2);
-        V3 e1 = v0 - v1, e2 = v2 - v0, ng = cross(e1, e2);
-        V3 C = v0 - o, R = cross(d, C);
-        auto edot = [](V3 a, V3 b) { return a.x*b.x + (a.y*b.y + a.z*b.z); };
-        float den = edot(ng, d), absDen = std::fabs(den);
-        auto xs = [&](float a) { return den < 0.0f || (den == 0.0f && std::signbit(den)) ? -a : a; };
-        float U = xs(edot(R, e2)), V = xs(edot(R, e1));
-        if (!(den != 0.0f && U >= 0.0f && V >= 0.0f && U + V <= absDen)) return;
-        float T = xs(edot(ng, C));
-        if (!(T > absDen*tnear && T < absDen*best)) return;
-        best = T/absDen;
-    };
+    auto tri_test = [&](uint32_t t, const V3 &o, const V3 &d, float tnear, float &best) { host_triangle(tris[t], o, d, tnear, best); };
     uint32_t bad = 0; uint64_t visits = 0;
     std::vector<int32_t> stack;
     for (uint32_t r = 0; r < n_rays; ++r) {
@@ -1687,6 +1697,92 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
     }
     *mismatches = bad;
     if (node_visits) *node_visits = visits;
+    return TGB_OK;
+}
+
+// Host-only count of the any-hit shadow walk's work (no GPU).  Builds the tree over n triangles as tgb200_create builds a triangle
+// scene's (padding from the larger magnitude of the triangles and the camera position), its top-level cut and QNode4 layout, and
+// walks every query (8 floats: o, d, tnear, t_light) with the kernels' node and triangle arithmetic twice: as k_shadow_bvh walked
+// any-hit queries before (children sorted near-to-far, from the root) and as it walks them now (nearest child entered, the others
+// pushed unsorted, from the cut boxes the segment enters).  A query that enters no cut box is not walked: k_shadow_prep settles it.
+// out = 10 uint32 per query: cut mask, deepest stack of the walk from the cut, then per walk (root, cut): occluded, node visits,
+// LEAF trips, triangle tests.  *stack_need = the bound tgb200_create checks; TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the
+// traversal's stack), before any walk.
+int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *camera_pos, const float *queries, uint32_t n_queries,
+                             uint32_t stack_size, uint32_t *stack_need, uint32_t *out) {
+    if (!tri_verts || n == 0 || !camera_pos || (n_queries && (!queries || !out))) return TGB_ERR_INVALID;
+    std::vector<BuildTri> tris(n);
+    float extent = std::max(std::max(std::fabs(camera_pos[0]), std::fabs(camera_pos[1])), std::fabs(camera_pos[2]));
+    for (uint32_t i = 0; i < n; ++i) { std::memcpy(&tris[i], tri_verts + 9*size_t(i), sizeof(BuildTri)); for (int k = 0; k < 9; ++k) extent = std::max(extent, std::fabs(tri_verts[9*size_t(i) + k])); }
+    Bvh4 bvh; build_bvh4(tris.data(), n, bvh, 0, 1e-6f*extent, 4, 0.5f);
+    const std::vector<CutBox> cut = top_level_cut(bvh, 16);
+    const uint32_t need = traversal_stack_need(bvh, cut);
+    if (stack_need) *stack_need = need;
+    if (need > (stack_size ? stack_size : uint32_t(kStackSize))) return TGB_ERR_UNSUPPORTED;
+    QBvh4 qb; quantize_bvh4(bvh, qb, ~int32_t(n << 3));
+    std::vector<int32_t> new_index(qb.old_index.size()), cut_link(cut.size());
+    for (size_t i = 0; i < qb.old_index.size(); ++i) new_index[size_t(qb.old_index[i])] = int32_t(i);
+    for (size_t i = 0; i < cut.size(); ++i) cut_link[i] = cut[i].link >= 0 ? new_index[size_t(cut[i].link)] : cut[i].link;
+    std::vector<int32_t> stack;
+    for (uint32_t r = 0; r < n_queries; ++r) {
+        const float *q = queries + 8*size_t(r);
+        const V3 o = f3(q), d = f3(q + 3); const float tnear = q[6], tfar = q[7];
+        const float ooeps = 1e-30f;
+        const float inv[3] = {1.0f/(std::fabs(d.x) > ooeps ? d.x : std::copysign(ooeps, d.x)), 1.0f/(std::fabs(d.y) > ooeps ? d.y : std::copysign(ooeps, d.y)),
+                              1.0f/(std::fabs(d.z) > ooeps ? d.z : std::copysign(ooeps, d.z))};
+        const float oo[3] = {o.x, o.y, o.z}, ood[3] = {o.x*inv[0], o.y*inv[1], o.z*inv[2]};
+        uint32_t mask = 0;                                                  // mesh_cut_test<true>
+        for (size_t k = 0; k < cut.size(); ++k) {
+            float tmn = tnear, tmx = tfar;
+            for (int a = 0; a < 3; ++a) {
+                const float ta = std::fmaf(cut[k].lo[a], inv[a], -ood[a]), tb = std::fmaf(cut[k].hi[a], inv[a], -ood[a]);
+                tmn = std::fmax(tmn, std::fmin(ta, tb)); tmx = std::fmin(tmx, std::fmax(ta, tb));
+            }
+            if (tmn <= tmx) mask |= 1u << k;
+        }
+        uint32_t *o10 = out + 10*size_t(r);
+        std::memset(o10, 0, 10*sizeof(uint32_t));
+        o10[0] = mask;
+        if (!mask) continue;
+        for (int from_cut = 0; from_cut < 2; ++from_cut) {
+            uint32_t *c4 = o10 + 2 + 4*from_cut;
+            stack.clear();
+            if (from_cut) { for (int k = int(cut.size()) - 1; k >= 0; --k) if (mask & (1u << k)) stack.push_back(cut_link[size_t(k)]); }
+            else stack.push_back(0);
+            bool occluded = false;
+            int32_t cur = stack.back(); stack.pop_back();
+            size_t deepest = stack.size();
+            for (;;) {
+                if (cur >= 0) {
+                    float t[4]; c4[1]++;
+                    qnode_slab_host(qb.nodes[size_t(cur)], oo, inv, tnear, tfar, t);
+                    int32_t l[4] = {qb.nodes[size_t(cur)].link[0], qb.nodes[size_t(cur)].link[1], qb.nodes[size_t(cur)].link[2], qb.nodes[size_t(cur)].link[3]};
+                    auto cswap = [&](int a, int b) { if (t[b] < t[a]) { std::swap(t[a], t[b]); std::swap(l[a], l[b]); } };
+                    cswap(0, 1); cswap(2, 3); cswap(0, 2);
+                    if (!from_cut) { cswap(1, 3); cswap(1, 2); }
+                    if (t[0] != INFINITY) {
+                        for (int k = 3; k >= 1; --k) if (t[k] != INFINITY) stack.push_back(l[k]);
+                        deepest = std::max(deepest, stack.size());
+                        cur = l[0];
+                        continue;
+                    }
+                } else {
+                    const int code = ~cur; const uint32_t first = uint32_t(code >> 3), count = uint32_t(code & 3) + 1;
+                    c4[2]++;
+                    for (uint32_t i = 0; i < count && !occluded; ++i) {
+                        c4[3]++;
+                        float best = tfar;
+                        if (first + i < n) occluded = host_triangle(tris[bvh.order[first + i]], o, d, tnear, best);
+                    }
+                    if (occluded) break;
+                }
+                if (stack.empty()) break;
+                cur = stack.back(); stack.pop_back();
+            }
+            c4[0] = occluded ? 1u : 0u;
+            if (from_cut) o10[1] = uint32_t(deepest);
+        }
+    }
     return TGB_OK;
 }
 
@@ -1834,19 +1930,15 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
     // one scratch slot per query: chunks of the context's capacity
     for (uint32_t off = 0; off < n && e == cudaSuccess; off += c->capacity) {
         const uint32_t m = std::min(c->capacity, n - off);
-        // shadow_count, shadow_count2, cursor_trace, cursor_shadow
-        e = cudaMemsetAsync(&c->ctl->shadow_count, 0, 4*sizeof(uint32_t), st);
+        // shadow_count, shadow_count2, cursor_trace, cursor_shadow, shadow_count_closest, cursor_closest
+        e = cudaMemsetAsync(&c->ctl->shadow_count, 0, 6*sizeof(uint32_t), st);
         if (e != cudaSuccess) break;
         k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, c->sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
                                                             c->squeue, c->ctl, m);
-        if (curves) k_shadow_prep<true><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->ctr);
-        else k_shadow_prep<false><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->ctr);
-        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(c->squeue2, c->ctl, dout + 8*size_t(off));
-        if (sc.n_nodes) {
-            const uint32_t grid = std::min(blocks(m, kTraceBlock), c->persist_blocks);
-            if (curves) k_shadow_bvh<true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
-            else k_shadow_bvh<false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->ctl, c->ctr);
-        }
+        if (curves) k_shadow_prep<true><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
+        else k_shadow_prep<false><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
+        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(c->squeue2, c->squeue_cl, c->ctl, dout + 8*size_t(off));
+        if (sc.n_nodes) launch_shadow_bvh(c, std::min(blocks(m, kTraceBlock), c->persist_blocks));
         k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(c->sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
         e = cudaGetLastError();
     }

@@ -136,6 +136,9 @@ struct DScene {
     // A ray that misses all of them is answered by the kernel that creates it and never reaches a traversal kernel.
     // (8-byte aligned: mesh_cut_hit reads two boxes' planes per 64-bit load from the kernel parameters)
     int n_cut; alignas(8) float cut[6][16];        // lo.x, hi.x, lo.y, hi.y, lo.z, hi.z
+    // where an any-hit shadow query enters the tree: the QNode4 index (or leaf code) below each cut box; cut_entry = 0 starts
+    // every query at the root instead (TGB_SHADOW_CUT_ENTRY=0, for A/B comparisons)
+    int32_t cut_link[16]; int cut_entry;
     V3 bin_lo, bin_inv;         // ray-binning grid over the scene bounds: cell = (o - bin_lo)*bin_inv, 16 cells per axis
     const uint32_t *sobol;      // 1024 x 32 direction matrices
 };

@@ -125,9 +125,10 @@ __global__ void __launch_bounds__(128) k_probe_shadow_setup(DScene sc, Scratch s
     o[6] = queued ? 1.0f : 0.0f; o[7] = any ? 1.0f : 0.0f;
 }
 // after k_shadow_prep: queued = 2 for the queries it left to k_shadow_bvh (the others it settled itself)
-__global__ void __launch_bounds__(256) k_probe_shadow_traversed(const uint32_t *squeue2, const Ctl *ctl, float *out) {
+__global__ void __launch_bounds__(256) k_probe_shadow_traversed(const uint32_t *squeue2, const uint32_t *squeue_cl, const Ctl *ctl, float *out) {
     const uint32_t j = blockIdx.x*blockDim.x + threadIdx.x;
     if (j < ctl->shadow_count2) out[8*size_t(squeue2[j] >> 2) + 6] = 2.0f;
+    if (j < ctl->shadow_count_closest) out[8*size_t(squeue_cl[j] >> 2) + 6] = 2.0f;
 }
 // after k_shadow_bvh: vis and the finished lightF (NEE) / bsdfF (MIS) of each query
 __global__ void __launch_bounds__(128) k_probe_shadow_read(Scratch sr, const int *light_mis, float *out, uint32_t n) {

@@ -44,7 +44,8 @@ struct Scratch {
     float4 *M0, *M1;    // MIS: (direction, pdfB | t of the light's own hit), (weight | finished bsdfF, NEE's pdfB)
     float4 *D0, *D1;    // (throughput before the bounce, light-pick weight), (surface emission term, light primitive)
     uint32_t *vis;      // vis[2s + mis] = 1 when that query's light term counts (nothing but the light in the way)
-    float4 *SH;         // per shadow-queue entry: the initial (analytic) hit of a closest-hit query
+    float4 *SH;         // per closest-hit shadow-queue entry: the query's initial (analytic) hit
+    uint32_t *cut_mask; // per any-hit shadow-queue entry: the top-level cut boxes its segment enters (bit k = DScene::cut box k)
     float4 *R;          // finished radiance per path of the step, indexed by path id (not by slot)
 };
 
@@ -67,8 +68,9 @@ struct Ctl {
     uint32_t capacity;
     uint32_t next_count;    // survivors appended by k_accum
     uint32_t shadow_count;  // NEE/MIS queries emitted by k_shade
-    uint32_t shadow_count2; // ... of which k_shadow_prep could not resolve analytically: the queue of k_shadow_bvh
+    uint32_t shadow_count2; // ... of which k_shadow_prep could not resolve analytically, any-hit: k_shadow_bvh's first queue
     uint32_t cursor_trace, cursor_shadow;       // ray cursors of the persistent traversal kernels
+    uint32_t shadow_count_closest, cursor_closest;    // ... closest-hit (mesh-light) ones: its second queue, and its cursor
     unsigned long long traversed, shadow_traversed;   // statistics: queries that reached k_trace / k_shadow_bvh
     uint32_t iterations;
 };
@@ -283,7 +285,8 @@ struct TravStack {
 // Node visit (QNode4, bvh_build.h) = 4 x 16-byte loads from global memory,
 // per axis a = S/d, b = (origin - o)/d - a once per node, then per child plane ONE byte permute (1 + q*2^-15 assembled
 // straight into float bits) and ONE fma; the hit children are ordered near-to-far with a 5-exchange sorting network, the
-// nearest is entered and the others are pushed far-to-near (three predicated shared-memory stores).
+// nearest is entered and the others are pushed far-to-near (three predicated shared-memory stores).  The any-hit walk stops the
+// network after the 3 exchanges that find the nearest and pushes the others unsorted.
 // Triangle test = Embree's MoellerTrumboreIntersector1 (thirdparty/embree/kernels/geometry/
 // triangle_intersector_moeller.h:75-111) with IEEE division for t,u,v.
 // `any`: occlusion query, stop at the first triangle hit.
@@ -415,7 +418,11 @@ struct Traversal {
 #define TGB_TRI_REFILL_IDLE 16
 #endif
 enum : int { CM_IDLE = 0, CM_NODE = 1, CM_LEAF = 2, CM_BISECT = 3, CM_CYL = 4 };
-template <bool CURVES, class P>
+// ANY (k_shadow_bvh's any-hit queries only): an occlusion query's answer -- is there any primitive in [tnear, t_light]? -- does not
+// depend on the order of its node visits nor on where its walk starts, so this walk skips the near-to-far sort (the nearest hit child
+// is entered, the others are pushed unsorted) and starts below the top-level cut (pol.enter pushes the subtrees of the cut boxes the
+// segment enters).  A closest-hit walk cannot do either: the visiting order decides which of two equally distant hits wins.
+template <bool CURVES, bool ANY = false, class P>
 TGB_D void bvh_traverse_persistent(const DScene &sc, int *smem_stack, P &pol, uint32_t n, uint32_t *counter) {
     const unsigned FULL = 0xffffffffu, lane = threadIdx.x & 31u;
     Traversal<CURVES> tr; TravStack stk; stk.base = smem_addr(smem_stack + threadIdx.x); int sp = 0;
@@ -467,7 +474,10 @@ TGB_D void bvh_traverse_persistent(const DScene &sc, int *smem_stack, P &pol, ui
             exhausted = first_ray + cnt >= n;
             if (mode == CM_IDLE && rank < cnt && first_ray + rank < n) {
                 V3 o, d; float tnear; Hit h; bool any;
-                if (pol.fetch(first_ray + rank, o, d, tnear, h, any)) { tr.begin(o, d, tnear, any, h); tr.ignore = pol.ignore(); sp = 0; mode = CM_NODE; }
+                if (pol.fetch(first_ray + rank, o, d, tnear, h, any)) {
+                    tr.begin(o, d, tnear, any, h); tr.ignore = pol.ignore(); sp = 0; mode = CM_NODE;
+                    if constexpr (ANY) { pol.enter(stk, sp); pop_node(); }
+                }
             }
             continue;
         }
@@ -516,10 +526,12 @@ TGB_D void bvh_traverse_persistent(const DScene &sc, int *smem_stack, P &pol, ui
                 float t0, t1, t2, t3; int4 lk;
                 tr.visit(sc, t0, t1, t2, t3, lk);
                 int l0 = lk.x, l1 = lk.y, l2 = lk.z, l3 = lk.w;
-                TGB_CSWAP(t0, l0, t1, l1) TGB_CSWAP(t2, l2, t3, l3) TGB_CSWAP(t0, l0, t2, l2) TGB_CSWAP(t1, l1, t3, l3) TGB_CSWAP(t1, l1, t2, l2)
+                // the first three exchanges leave the nearest child in slot 0; the last two sort the other three
+                TGB_CSWAP(t0, l0, t1, l1) TGB_CSWAP(t2, l2, t3, l3) TGB_CSWAP(t0, l0, t2, l2)
+                if (!ANY) { TGB_CSWAP(t1, l1, t3, l3) TGB_CSWAP(t1, l1, t2, l2) }
                 if (t0 == INFINITY) pop_node();
                 else {
-                    // sorted, so the children to push are a prefix of (l1, l2, l3); the nearest of them must end up on top
+                    // closest hit: sorted, so the nearest of the pushed children ends up on top
                     const bool p1 = t1 != INFINITY, p2 = t2 != INFINITY, p3 = t3 != INFINITY;
                     if (sp + 3 <= kSmemStack) {
                         const uint32_t a3 = stk.base + uint32_t(sp)*(kTraceBlock*4u);
@@ -583,14 +595,15 @@ TGB_D void bvh_traverse_persistent(const DScene &sc, int *smem_stack, P &pol, ui
 
 // Coherent pre-test of a new ray against the BVH's top-level cut (DScene::cut), with fused slab arithmetic on the float
 // boxes the tree was built from (the quantised node boxes contain them): false means every subtree would be culled, i.e.
-// the query's answer is the ray's analytic hit.
-TGB_D bool mesh_cut_hit(const DScene &sc, V3 o, V3 d, float tnear, float tfar) {
+// the query's answer is the ray's analytic hit.  MASK: the set of boxes entered instead (bit k = box k), where an any-hit walk starts.
+template <bool MASK>
+TGB_D uint32_t mesh_cut_test(const DScene &sc, V3 o, V3 d, float tnear, float tfar) {
     const float ooeps = 1e-30f;
     const float idx = 1.0f/(fabsf(d.x) > ooeps ? d.x : copysignf(ooeps, d.x));
     const float idy = 1.0f/(fabsf(d.y) > ooeps ? d.y : copysignf(ooeps, d.y));
     const float idz = 1.0f/(fabsf(d.z) > ooeps ? d.z : copysignf(ooeps, d.z));
     const float oodx = o.x*idx, oody = o.y*idy, oodz = o.z*idz;
-    bool hit = false;
+    bool hit = false; uint32_t mask = 0;
     // groups of four boxes with static indices inside a group (the boxes are read straight from the kernel parameters); the
     // number of groups is uniform across the grid
 #pragma unroll
@@ -604,12 +617,14 @@ TGB_D bool mesh_cut_hit(const DScene &sc, V3 o, V3 d, float tnear, float tfar) {
                 float az = __fmaf_rn(sc.cut[4][k], idz, -oodz), bz = __fmaf_rn(sc.cut[5][k], idz, -oodz);
                 float tmn = fmaxf(fmaxf(fminf(ax, bx), fminf(ay, by)), fmaxf(fminf(az, bz), tnear));
                 float tmx = fminf(fminf(fmaxf(ax, bx), fmaxf(ay, by)), fminf(fmaxf(az, bz), tfar));
-                hit = hit || (k < sc.n_cut && tmn <= tmx);
+                if (MASK) mask |= (k < sc.n_cut && tmn <= tmx) ? 1u << k : 0u;
+                else hit = hit || (k < sc.n_cut && tmn <= tmx);
             }
         }
     }
-    return hit;
+    return MASK ? mask : uint32_t(hit);
 }
+TGB_D bool mesh_cut_hit(const DScene &sc, V3 o, V3 d, float tnear, float tfar) { return mesh_cut_test<false>(sc, o, d, tnear, tfar) != 0; }
 
 // Fill a Surface from a hit: Primitive::intersectionInfo for mesh/quad/cube
 // (TriangleMesh.cpp:323-331,344-355; Quad.cpp:112-120; Cube.cpp:157-171) + TraceableScene::intersect (:183-188)
@@ -1218,21 +1233,25 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
 // Analytic part of the NEE/MIS queries (quads and cubes are tested coherently, every lane runs the same loop), top-level
 // BVH cut, and compaction of what is left for k_shadow_bvh.  (Fusing this into k_shade's tail was measured (B200): the 13 values it
 // needs stay live across the BSDF code, k_shade spills and gets slower than both kernels together.)
+// The queries left for the BVH are compacted into two queues, so that every warp of k_shadow_bvh runs one kind: any-hit queries
+// (quad / cap / environment lights) into squeue2 with the mask of the cut boxes they enter, closest-hit (mesh-light) queries into
+// squeue_cl with their analytic hit.
 template <bool CURVES>
-__global__ void __launch_bounds__(256) k_shadow_prep(DScene sc, Scratch sr, const uint32_t *squeue, Ctl *ctl, uint32_t *squeue2, Counters *ctr) {
+__global__ void __launch_bounds__(256) k_shadow_prep(DScene sc, Scratch sr, const uint32_t *squeue, Ctl *ctl, uint32_t *squeue2,
+                                                     uint32_t *squeue_cl, Counters *ctr) {
     uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
     bool valid = i < ctl->shadow_count;
-    bool keep = false, blocked = false; uint32_t q = 0; Hit h; h.t = INFINITY; h.u = h.v = 0.0f; h.id = HID_MISS;
+    bool keep = false, blocked = false, any = false; uint32_t q = 0, cut = 0; Hit h; h.t = INFINITY; h.u = h.v = 0.0f; h.id = HID_MISS;
     if (valid) {
         q = squeue[i];
-        uint32_t s = q >> 2; bool mis = q & 1u, any = q & 2u;
+        uint32_t s = q >> 2; bool mis = q & 1u; any = q & 2u;
         const float4 P = sr.P[s], D = mis ? sr.M0[s] : sr.N0[s];
         V3 p = v3(P.x, P.y, P.z), d = v3(D.x, D.y, D.z);
         const float eps = P.w;                                        // info.epsilon of the shading point (TraceBase.cpp:254,295)
         if (any) {
             const int li = __float_as_int(sr.D1[s].w);
             blocked = analytic_any(sc, p, d, eps, D.w, li);
-            if (!blocked) { if (!mesh_cut_hit(sc, p, d, eps, D.w)) sr.vis[2*size_t(s) + (mis ? 1 : 0)] = 1u; else keep = true; }
+            if (!blocked) { cut = mesh_cut_test<true>(sc, p, d, eps, D.w); if (!cut) sr.vis[2*size_t(s) + (mis ? 1 : 0)] = 1u; else keep = true; }
         } else {
             h = analytic_closest(sc, p, d, eps, INFINITY);
             if (!mesh_cut_hit(sc, p, d, eps, h.t)) blocked = h.id != HID_MISS;       // an analytic primitive is never the (mesh) light: not visible
@@ -1240,49 +1259,71 @@ __global__ void __launch_bounds__(256) k_shadow_prep(DScene sc, Scratch sr, cons
         }
     }
     count_block(&ctr->shadow_rays, &ctr->shadow_hits, valid, blocked);
-    unsigned m = __ballot_sync(0xffffffffu, keep);
-    if (m) {
-        unsigned lane = threadIdx.x & 31, base = 0;
-        if (lane == 0) base = atomicAdd(&ctl->shadow_count2, unsigned(__popc(m)));
+    const unsigned lane = threadIdx.x & 31, lt = (1u << lane) - 1u;
+    const unsigned ma = __ballot_sync(0xffffffffu, keep && any), mc = __ballot_sync(0xffffffffu, keep && !any);
+    if (ma) {
+        unsigned base = 0;
+        if (lane == 0) base = atomicAdd(&ctl->shadow_count2, unsigned(__popc(ma)));
         base = __shfl_sync(0xffffffffu, base, 0);
-        if (keep) {
-            uint32_t at = base + __popc(m & ((1u << lane) - 1u));
-            squeue2[at] = q;
-            if (!(q & 2u)) sr.SH[at] = pack_hit(h);
-        }
+        if (keep && any) { const uint32_t at = base + __popc(ma & lt); squeue2[at] = q; sr.cut_mask[at] = cut; }
+    }
+    if (mc) {
+        unsigned base = 0;
+        if (lane == 0) base = atomicAdd(&ctl->shadow_count_closest, unsigned(__popc(mc)));
+        base = __shfl_sync(0xffffffffu, base, 0);
+        if (keep && !any) { const uint32_t at = base + __popc(mc & lt); squeue_cl[at] = q; sr.SH[at] = pack_hit(h); }
     }
 }
 
-template <bool CURVES>
+// ANY: the queue of any-hit queries (squeue2), else that of closest-hit queries (squeue_cl)
+template <bool CURVES, bool ANY>
 struct ShadowPolicy {
     DScene sc; Scratch sr; const uint32_t *squeue; unsigned long long *hits;
-    uint32_t s; bool mis, any; int li, ign; V3 p, d;
+    uint32_t s, cut; bool mis; int li, ign; V3 p, d;
     TGB_D bool fetch(uint32_t i, V3 &o, V3 &dd, float &tnear, Hit &h, bool &anyq) {
         uint32_t q = squeue[i];
-        s = q >> 2; mis = q & 1u; any = q & 2u;
+        s = q >> 2; mis = q & 1u;
         const float4 P = sr.P[s], D = mis ? sr.M0[s] : sr.N0[s];
         p = v3(P.x, P.y, P.z); d = v3(D.x, D.y, D.z);
-        o = p; dd = d; tnear = P.w; anyq = any; li = 0;
-        if (any) {
+        o = p; dd = d; tnear = P.w; anyq = ANY; li = 0;
+        if (ANY) {
             h.t = D.w; h.u = 0.0f; h.v = 0.0f; h.id = HID_MISS;
             // analytic primitives in the BVH: the query must not count the light it is aimed at (generalizedShadowRay's
             // `hit == endCap`, TraceBase.cpp:79-83); with the usual per-ray loop k_shadow_prep has dealt with them already
             ign = sc.n_analytic == 0 && sc.analytic_base != 0x7fffffff ? __float_as_int(sr.D1[s].w) : -1;
+            cut = sr.cut_mask[i];
         } else { h = unpack_hit(sr.SH[i]); li = __float_as_int(sr.D1[s].w); ign = -1; }
         return true;
+    }
+    // any-hit walk: start in the subtrees of the cut boxes the segment enters, box 0 first (a segment that enters none never
+    // gets here, and no primitive outside the cut boxes can block it)
+    TGB_D void enter(TravStack &stk, int &sp) const {
+        if (!sc.cut_entry) { stk.push(sp, 0); return; }
+#pragma unroll
+        for (int k = 15; k >= 0; --k) if (cut & (1u << k)) stk.push(sp, sc.cut_link[k]);
     }
     TGB_D int ignore() const { return ign; }
     TGB_D void finish(const Hit &h) {
         if (h.id != HID_MISS) atomicAdd(hits, 1ull);
-        if (any) { if (h.id == HID_MISS) sr.vis[2*size_t(s) + (mis ? 1 : 0)] = 1u; }
+        if (ANY) { if (h.id == HID_MISS) sr.vis[2*size_t(s) + (mis ? 1 : 0)] = 1u; }
         else shadow_resolve_closest<CURVES>(sc, sr, s, mis, li, p, d, h);
     }
 };
-template <bool CURVES>
-__global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_shadow_bvh(DScene sc, Scratch sr, const uint32_t *squeue, Ctl *ctl, Counters *ctr) {
+// One launch for both queues: a warp walks any-hit queries until that queue is exhausted and its lanes are done, then (scenes with
+// mesh lights) closest-hit ones, so the end of the first walk overlaps other warps' second and the launch has one drain tail.
+// (Two launches, one per queue, measured 2.7 % slower on C2, H100: a second tail per iteration.)
+template <bool CURVES, bool MESH_LIGHTS>
+__global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_shadow_bvh(DScene sc, Scratch sr, const uint32_t *squeue2,
+                                                                                                const uint32_t *squeue_cl, Ctl *ctl, Counters *ctr) {
     __shared__ int smem_stack[kSmemStack*kTraceBlock];
-    ShadowPolicy<CURVES> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue; pol.hits = &ctr->shadow_hits;
-    bvh_traverse_persistent<CURVES>(sc, smem_stack, pol, ctl->shadow_count2, &ctl->cursor_shadow);
+    {
+        ShadowPolicy<CURVES, true> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue2; pol.hits = &ctr->shadow_hits;
+        bvh_traverse_persistent<CURVES, true>(sc, smem_stack, pol, ctl->shadow_count2, &ctl->cursor_shadow);
+    }
+    if (MESH_LIGHTS) {
+        ShadowPolicy<CURVES, false> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue_cl; pol.hits = &ctr->shadow_hits;
+        bvh_traverse_persistent<CURVES, false>(sc, smem_stack, pol, ctl->shadow_count_closest, &ctl->cursor_closest);
+    }
 }
 
 // Fold this bounce's direct light + surface emission into the path (order as in handleSurface:537-543), apply the
@@ -1389,13 +1430,14 @@ __global__ void __launch_bounds__(1024) k_iter_end(uint32_t *hist, Ctl *ctl, int
     }
     __syncthreads();
     if (t == 0) {
-        if (has_bvh) { ctl->traversed += (unsigned long long)ctl->n_sorted + ctl->n_new; ctl->shadow_traversed += ctl->shadow_count2; }
+        if (has_bvh) { ctl->traversed += (unsigned long long)ctl->n_sorted + ctl->n_new; ctl->shadow_traversed += ctl->shadow_count2 + ctl->shadow_count_closest; }
         ctl->iterations++;
         const uint32_t n_surv = ctl->next_count;
         const uint32_t n_new = min(ctl->capacity - n_surv, ctl->total - ctl->issued);
         ctl->first_path = ctl->issued; ctl->issued += n_new;
         ctl->n_surv = n_surv; ctl->n_new = n_new; ctl->n = n_surv + n_new; ctl->n_sorted = total_sorted;
         ctl->next_count = 0u; ctl->shadow_count = 0u; ctl->shadow_count2 = 0u; ctl->cursor_trace = 0u; ctl->cursor_shadow = 0u;
+        ctl->shadow_count_closest = 0u; ctl->cursor_closest = 0u;
     }
 }
 // ... and scatter of the slot indices (4 bytes each) to their sorted positions.

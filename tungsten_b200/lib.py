@@ -47,6 +47,7 @@ def load():
     L.tgb200_abort.argtypes = [vp]
     L.tgb200_clear_abort.argtypes = [vp]
     L.tgb200_qbvh_selftest.argtypes = [vp, u32, vp, u32, C.POINTER(u32), C.POINTER(u32), C.POINTER(C.c_uint64)]
+    L.tgb200_shadow_walk_count.argtypes = [vp, u32, vp, vp, u32, u32, C.POINTER(u32), vp]
     i32, f32 = C.c_int, C.c_float
     L.tgb200_bsdf_probe.argtypes = [vp, i32, f32, f32, u32, i32, u32, vp, vp]
     L.tgb200_bsdf_sample_probe.argtypes = [vp, u32, u32, vp, vp, u32, f32, f32, u32, i32, vp, vp, vp]
