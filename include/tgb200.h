@@ -258,10 +258,13 @@ int tgb200_shard_tiles(const tgb_tile *tiles, uint32_t n_tiles, uint32_t *order)
 int tgb200_trace_closest(tgb_ctx *ctx, const tgb_ray *rays, tgb_hit *hits, uint32_t n);
 
 int  tgb200_get_stats(tgb_ctx *ctx, tgb_stats *out);
-/* Time every kernel of the wavefront loop with CUDA events on the render stream (fills the *_ms fields of tgb_stats). */
+/* Time every kernel of the wavefront loop with CUDA events on the streams of both wavefronts (fills the *_ms fields of
+ * tgb_stats with sums over both; their kernels overlap, so the sums do not add up to total_ms).                         */
 int  tgb200_set_profiling(tgb_ctx *ctx, int enable);
 /* Run the context's work on the caller's CUDA stream (a cudaStream_t; NULL = back to the context's own stream), so that a
- * caller's events and collectives on that stream order with the renders.                                           */
+ * caller's events and collectives on that stream order with the renders.  A render runs its second wavefront on a stream
+ * of the context's own, forked from the caller's stream at its start and joined back into it before the framebuffer is
+ * written: work queued on the caller's stream after the call sees the finished render.                               */
 int  tgb200_set_stream(tgb_ctx *ctx, void *cuda_stream);
 /* Size of what was built: triangles, BVH nodes, BVH depth, bytes of nodes+triangle records, and the
  * wavefront capacity (paths in flight).  Any pointer may be NULL.                                   */
@@ -309,7 +312,7 @@ int  tgb200_choose_light_probe(tgb_ctx *ctx, uint32_t seed, uint32_t n, const ui
  * (point p.xyz, direction d.xyz, epsilon, arg) + 2 ints light_mis = (light primitive, mis).  A NEE query (mis = 0, arg = the
  * expected distance) is set up as the shading kernel sets up lightSample's with f = 1, pdfL = 1, pdfB = 0; a MIS query (mis = 1,
  * arg = the BSDF pdf) as bsdfSample's with weight = 1.  Then the analytic / cut pass and the BVH pass run as in a render, in
- * chunks of the context's capacity.  out = 8 floats per query: light hit (mesh lights: 1), t of the light (mesh lights: 0), vis,
+ * chunks of half the context's capacity (the path slots of its first wavefront).  out = 8 floats per query: light hit (mesh lights: 1), t of the light (mesh lights: 0), vis,
  * the finished lightF / bsdfF rgb (emission, or emission x the power heuristic for MIS; counts only when vis = 1), queued
  * (0: no query, 1: settled by the analytic / cut pass, 2: reached the BVH pass), traced as a blocker test.  A failed probe
  * still restores them unless the device itself faulted.  The context's control block and ray counters are left as they were. */

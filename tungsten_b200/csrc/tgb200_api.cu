@@ -45,34 +45,43 @@ struct DeviceBuf {
     void *p = nullptr; size_t bytes = 0;
 };
 
+// One wavefront: the loop state of its share of a (sub)step's camera paths.  A context runs two of them, each on its own stream,
+// so that one wavefront's traversal kernels (ALU bound) run alongside the other's streaming kernels (HBM bound).
+struct Wavefront {
+    uint32_t capacity = 0;          // path slots: half of the context's capacity
+    PathBuf pb[2]{};                // persistent path state, double buffered (k_accum compacts from one into the other)
+    Scratch sr{};                   // per-bounce scratch records; sr.R is the context's result buffer, shared by both wavefronts
+    uint32_t *order = nullptr, *squeue = nullptr, *squeue2 = nullptr;   // ray-coherence visiting order of k_trace; shadow-query queues (emitted / left after the analytic pass)
+    uint32_t *squeue_cl = nullptr;  // ... the closest-hit (mesh-light) queries left after the analytic pass
+    uint32_t *bin_keys = nullptr, *bin_hist = nullptr;
+    Ctl *ctl = nullptr;             // device-resident loop control block
+    Ctl *h_ctl = nullptr;           // pinned: [0..3] snapshot ring (read one iteration late), [4] initial value
+    cudaEvent_t ev_ring[4]{};
+    cudaEvent_t ev_k[4][8]{};       // profiling: boundaries between the kernels of an iteration (regen|trace|shade|prep|shadow|accum|sort)
+};
+
 }  // namespace
 
 struct tgb_ctx {
     int device = 0;
-    cudaStream_t stream = nullptr;
+    cudaStream_t stream = nullptr;  // the caller's stream (tgb200_set_stream) or own_stream: wavefront 0, k_resolve, the hooks
+    cudaStream_t stream1 = nullptr; // wavefront 1
+    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     std::string error;
     std::atomic<int> abort_flag{0};
     std::vector<void *> allocs;
     DScene sc{};
     uint32_t res_x = 0, res_y = 0;
     // wavefront storage
-    uint32_t capacity = 0;
-    PathBuf pb[2]{};                // persistent path state, double buffered (k_accum compacts from one into the other)
-    Scratch sr{};                   // per-bounce scratch records + per-step results
-    uint32_t *order = nullptr, *squeue = nullptr, *squeue2 = nullptr;   // ray-coherence visiting order of k_trace; shadow-query queues (emitted / left after the analytic pass)
-    uint32_t *squeue_cl = nullptr;  // ... the closest-hit (mesh-light) queries left after the analytic pass
+    uint32_t capacity = 0;          // paths in flight, both wavefronts together
+    Wavefront wf[2];                // the hooks run on wf[0]'s buffers
     bool mesh_lights = false;       // a mesh is a light: closest-hit shadow queries exist, k_shadow_bvh<., false> runs
-    uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels
+    uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels (per wavefront)
     bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
     bool has_curves = false;        // selects the kernel instantiations with the curve-segment test and per-hit epsilon
     int n_bsdfs = 0; std::vector<uint32_t> prim_types; std::vector<int> light_ids;   // host copies for the test hooks' argument checks
-    uint32_t *bin_keys = nullptr, *bin_hist = nullptr;
-    size_t res_capacity = 0;
-    Ctl *ctl = nullptr;             // device-resident loop control block
-    Ctl *h_ctl = nullptr;           // pinned: [0..3] snapshot ring (read one iteration late), [4] initial value
-    cudaEvent_t ev_ring[4]{};
-    cudaEvent_t ev_k[4][8]{};       // profiling: boundaries between the kernels of an iteration (regen|trace|shade|prep|shadow|accum|sort)
+    float4 *R = nullptr; size_t res_capacity = 0;   // finished radiance per path of the (sub)step
     cudaStream_t own_stream = nullptr;
     struct Group *group = nullptr;  // multi-GPU: set on the root context (devices[0]); members[0] == the root itself
     Counters *ctr = nullptr; Counters *h_ctr = nullptr;
@@ -706,27 +715,31 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
 int alloc_wavefront(tgb_ctx *c, uint32_t capacity) {
     c->capacity = capacity;
     int rc;
-    for (int k = 0; k < 2; ++k) {
-        for (float4 **p : {&c->pb[k].T0, &c->pb[k].T1, &c->pb[k].T2, &c->pb[k].T3}) if ((rc = dev_alloc(c, p, capacity))) return rc;
-        if ((rc = dev_alloc(c, &c->pb[k].E, capacity))) return rc;
-        if ((rc = dev_alloc(c, &c->pb[k].pcg, capacity))) return rc;
+    for (int h = 0; h < 2; ++h) {
+        Wavefront &w = c->wf[h];
+        const uint32_t cap = w.capacity = capacity/2 + (h == 0 ? capacity % 2 : 0);
+        for (int k = 0; k < 2; ++k) {
+            for (float4 **p : {&w.pb[k].T0, &w.pb[k].T1, &w.pb[k].T2, &w.pb[k].T3}) if ((rc = dev_alloc(c, p, cap))) return rc;
+            if ((rc = dev_alloc(c, &w.pb[k].E, cap))) return rc;
+            if ((rc = dev_alloc(c, &w.pb[k].pcg, cap))) return rc;
+        }
+        for (float4 **p : {&w.sr.P, &w.sr.N0, &w.sr.N1, &w.sr.M0, &w.sr.M1, &w.sr.D0, &w.sr.D1})
+            if ((rc = dev_alloc(c, p, cap))) return rc;
+        if ((rc = dev_alloc(c, &w.sr.vis, size_t(cap)*2))) return rc;
+        if ((rc = dev_alloc(c, &w.sr.SH, size_t(cap)*2))) return rc;
+        if ((rc = dev_alloc(c, &w.sr.cut_mask, size_t(cap)*2))) return rc;
+        if ((rc = dev_alloc(c, &w.squeue, size_t(cap)*2))) return rc;
+        if ((rc = dev_alloc(c, &w.squeue2, size_t(cap)*2))) return rc;
+        if ((rc = dev_alloc(c, &w.squeue_cl, size_t(cap)*2))) return rc;
+        if ((rc = dev_alloc(c, &w.order, cap))) return rc;
+        if ((rc = dev_alloc(c, &w.bin_keys, cap))) return rc;
+        if ((rc = dev_alloc(c, &w.bin_hist, size_t(kBins) + 4))) return rc;
+        if ((rc = dev_alloc(c, &w.ctl, 1))) return rc;
+        CU(cudaMemset(w.ctl, 0, sizeof(Ctl)));
+        CU(cudaMallocHost(reinterpret_cast<void **>(&w.h_ctl), 5*sizeof(Ctl)));
     }
-    for (float4 **p : {&c->sr.P, &c->sr.N0, &c->sr.N1, &c->sr.M0, &c->sr.M1, &c->sr.D0, &c->sr.D1})
-        if ((rc = dev_alloc(c, p, capacity))) return rc;
-    if ((rc = dev_alloc(c, &c->sr.vis, size_t(capacity)*2))) return rc;
-    if ((rc = dev_alloc(c, &c->sr.SH, size_t(capacity)*2))) return rc;
-    if ((rc = dev_alloc(c, &c->sr.cut_mask, size_t(capacity)*2))) return rc;
-    if ((rc = dev_alloc(c, &c->squeue, size_t(capacity)*2))) return rc;
-    if ((rc = dev_alloc(c, &c->squeue2, size_t(capacity)*2))) return rc;
-    if ((rc = dev_alloc(c, &c->squeue_cl, size_t(capacity)*2))) return rc;
-    if ((rc = dev_alloc(c, &c->order, capacity))) return rc;
-    if ((rc = dev_alloc(c, &c->bin_keys, capacity))) return rc;
-    if ((rc = dev_alloc(c, &c->bin_hist, size_t(kBins) + 4))) return rc;
-    if ((rc = dev_alloc(c, &c->ctl, 1))) return rc;
     if ((rc = dev_alloc(c, &c->ctr, 1))) return rc;
     CU(cudaMemset(c->ctr, 0, sizeof(Counters)));
-    CU(cudaMemset(c->ctl, 0, sizeof(Ctl)));
-    CU(cudaMallocHost(reinterpret_cast<void **>(&c->h_ctl), 5*sizeof(Ctl)));
     CU(cudaMallocHost(reinterpret_cast<void **>(&c->h_ctr), sizeof(Counters)));
     size_t npx = size_t(c->res_x)*c->res_y;
     if ((rc = dev_alloc(c, &c->fb, npx*3))) return rc;
@@ -789,64 +802,65 @@ inline unsigned blocks(uint32_t n, unsigned bs) { return n ? (n + bs - 1)/bs : 1
 // iteration traces a full batch until the step's paths run out (one drain tail per step instead of one per batch).
 int ensure_results(tgb_ctx *c, size_t n_paths) {
     if (n_paths <= c->res_capacity) return TGB_OK;
-    if (c->sr.R) cudaFree(c->sr.R);
-    c->sr.R = nullptr; c->res_capacity = 0;
-    CU(cudaMalloc(reinterpret_cast<void **>(&c->sr.R), n_paths*sizeof(float4)));
+    if (c->R) cudaFree(c->R);
+    c->R = nullptr; c->res_capacity = 0;
+    for (Wavefront &w : c->wf) w.sr.R = nullptr;
+    CU(cudaMalloc(reinterpret_cast<void **>(&c->R), n_paths*sizeof(float4)));
     c->res_capacity = n_paths;
+    for (Wavefront &w : c->wf) w.sr.R = c->R;
     return TGB_OK;
 }
 
 // k_shadow_bvh over the any-hit queue and (scenes with mesh lights) the closest-hit queue
-void launch_shadow_bvh(tgb_ctx *c, uint32_t grid) {
-    const DScene &sc = c->sc; cudaStream_t st = c->stream;
+void launch_shadow_bvh(tgb_ctx *c, const Wavefront &w, cudaStream_t st, uint32_t grid) {
+    const DScene &sc = c->sc;
     if (c->has_curves) {
-        if (c->mesh_lights) k_shadow_bvh<true, true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
-        else k_shadow_bvh<true, false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
+        if (c->mesh_lights) k_shadow_bvh<true, true><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
+        else k_shadow_bvh<true, false><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
     } else {
-        if (c->mesh_lights) k_shadow_bvh<false, true><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
-        else k_shadow_bvh<false, false><<<grid, kTraceBlock, 0, st>>>(sc, c->sr, c->squeue2, c->squeue_cl, c->ctl, c->ctr);
+        if (c->mesh_lights) k_shadow_bvh<false, true><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
+        else k_shadow_bvh<false, false><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
     }
 }
 
-// One iteration's kernels.  `bound` >= the iteration's ctl.n: grids are upper bounds, the kernels read the real sizes from
-// the device-resident control block.
-void enqueue_iteration(tgb_ctx *c, const BatchInfo &bi, int cur, uint32_t bound, int slot, uint64_t &launches) {
+// One iteration's kernels of wavefront w on stream st.  `bound` >= the iteration's ctl.n: grids are upper bounds, the kernels
+// read the real sizes from the device-resident control block.
+void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInfo &bi, int cur, uint32_t bound, int slot, uint64_t &launches) {
     const DScene &sc = c->sc;
     const bool has_bvh = sc.n_nodes != 0, curves = c->has_curves;
-    PathBuf &pb = c->pb[cur], &nxt = c->pb[cur ^ 1];
-    cudaStream_t st = c->stream;
+    PathBuf &pb = w.pb[cur], &nxt = w.pb[cur ^ 1];
     const bool prof = c->profiling;
-    if (prof) cudaEventRecord(c->ev_k[slot][0], st);
-    k_regen<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, bi, c->ctl, c->order, c->bin_hist); launches++;
-    if (prof) cudaEventRecord(c->ev_k[slot][1], st);
+    if (prof) cudaEventRecord(w.ev_k[slot][0], st);
+    k_regen<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
+    if (prof) cudaEventRecord(w.ev_k[slot][1], st);
     if (has_bvh) {
         uint32_t grid = std::min(blocks(bound, kTraceBlock), c->persist_blocks);
-        if (curves) k_trace<true><<<grid, kTraceBlock, 0, st>>>(sc, pb, c->order, c->ctl);
-        else k_trace<false><<<grid, kTraceBlock, 0, st>>>(sc, pb, c->order, c->ctl);
+        if (curves) k_trace<true><<<grid, kTraceBlock, 0, st>>>(sc, pb, w.order, w.ctl);
+        else k_trace<false><<<grid, kTraceBlock, 0, st>>>(sc, pb, w.order, w.ctl);
         launches++;
     }
-    if (prof) cudaEventRecord(c->ev_k[slot][2], st);
+    if (prof) cudaEventRecord(w.ev_k[slot][2], st);
     if (c->sort_materials) {
-        if (curves) k_shade<true, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, c->sr, bi, c->ctl, c->squeue, c->ctr);
-        else k_shade<false, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, c->sr, bi, c->ctl, c->squeue, c->ctr);
+        if (curves) k_shade<true, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
+        else k_shade<false, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     } else {
-        if (curves) k_shade<true, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, c->sr, bi, c->ctl, c->squeue, c->ctr);
-        else if (c->diffuse_only) k_shade<false, false, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, c->sr, bi, c->ctl, c->squeue, c->ctr);
-        else k_shade<false, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, c->sr, bi, c->ctl, c->squeue, c->ctr);
+        if (curves) k_shade<true, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
+        else if (c->diffuse_only) k_shade<false, false, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
+        else k_shade<false, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     }
     launches++;
-    if (prof) cudaEventRecord(c->ev_k[slot][3], st);
-    if (curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
-    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
+    if (prof) cudaEventRecord(w.ev_k[slot][3], st);
+    if (curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
     launches++;
-    if (prof) cudaEventRecord(c->ev_k[slot][4], st);
-    if (has_bvh) { launch_shadow_bvh(c, std::min(blocks(2*bound, kTraceBlock), c->persist_blocks)); launches++; }
-    if (prof) cudaEventRecord(c->ev_k[slot][5], st);
-    k_accum<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, nxt, c->sr, bi, c->ctl, c->bin_keys, c->bin_hist); launches++;
-    if (prof) cudaEventRecord(c->ev_k[slot][6], st);
-    k_iter_end<<<1, 1024, 0, st>>>(c->bin_hist, c->ctl, has_bvh ? 1 : 0); launches++;
-    if (has_bvh) { k_bin_scatter<<<blocks(bound, 256), 256, 0, st>>>(c->bin_keys, c->bin_hist, c->ctl, c->order); launches++; }
-    if (prof) cudaEventRecord(c->ev_k[slot][7], st);
+    if (prof) cudaEventRecord(w.ev_k[slot][4], st);
+    if (has_bvh) { launch_shadow_bvh(c, w, st, std::min(blocks(2*bound, kTraceBlock), c->persist_blocks)); launches++; }
+    if (prof) cudaEventRecord(w.ev_k[slot][5], st);
+    k_accum<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, nxt, w.sr, bi, w.ctl, w.bin_keys, w.bin_hist); launches++;
+    if (prof) cudaEventRecord(w.ev_k[slot][6], st);
+    k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, has_bvh ? 1 : 0); launches++;
+    if (has_bvh) { k_bin_scatter<<<blocks(bound, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order); launches++; }
+    if (prof) cudaEventRecord(w.ev_k[slot][7], st);
 }
 
 // `adaptive`: per-pixel sample ranges come from c->pix_first / c->pix_base (tgb200_render_adaptive), else every pixel
@@ -875,38 +889,64 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, bool adapt
         if (rc) return rc;
         BatchInfo bi; bi.pix_id = c->pix_id; bi.pix_seed = c->pix_seed; bi.n_pix = c->n_pix; bi.spp_begin = spp_begin + s0;
         bi.pix_first = adaptive ? c->pix_first : nullptr; bi.pix_base = adaptive ? c->pix_base : nullptr; bi.pix_bits = pix_bits;
-        // control block of the first iteration; from then on k_iter_end keeps it
-        Ctl &init = c->h_ctl[4];
-        std::memset(&init, 0, sizeof(Ctl));
-        init.capacity = c->capacity; init.total = total;
-        init.n_new = std::min(c->capacity, total); init.n = init.n_new; init.issued = init.n_new;
-        CU(cudaMemcpyAsync(c->ctl, &init, sizeof(Ctl), cudaMemcpyHostToDevice, c->stream));
-        // The host runs one iteration ahead of the device: after enqueueing iteration i it waits for the snapshot taken after
-        // iteration i-1 (normally long complete), which bounds the grids of iteration i+1 and tells when the step has drained.
-        uint32_t bound = init.n;                              // upper bound of ctl.n for the iteration about to be queued
-        int cur = 0;
-        for (uint32_t iter = 0;; ++iter) {
-            if (c->abort_flag.load()) { cudaStreamSynchronize(c->stream); c->abort_flag.store(0); return fail(c, TGB_ERR_ABORTED, "render aborted"); }
+        // fork: wavefront 1 starts behind what the caller's stream holds so far (the previous sub-step's k_resolve reads R)
+        const cudaStream_t st[2] = {c->stream, c->stream1};
+        CU(cudaEventRecord(c->ev_fork, st[0]));
+        CU(cudaStreamWaitEvent(st[1], c->ev_fork, 0));
+        // The (sub)step's path ids (result slots) are split statically: wavefront h issues the camera paths [base, end).  The
+        // image cannot depend on the split (every path seeds its own RNG and writes R[path id], DESIGN.md section 3).
+        const uint32_t half = total - total/2;
+        uint32_t bound[2] = {0, 0};                           // upper bound of ctl.n for the iteration about to be queued
+        int cur[2] = {0, 0};
+        bool live[2] = {false, false};
+        for (int h = 0; h < 2; ++h) {
+            Wavefront &w = c->wf[h];
+            const uint32_t base = h ? half : 0, end = h ? total : half;
+            if (end == base) continue;
+            // control block of the first iteration; from then on k_iter_end keeps it
+            Ctl &init = w.h_ctl[4];
+            std::memset(&init, 0, sizeof(Ctl));
+            init.capacity = w.capacity; init.total = end; init.first_path = base;
+            init.n_new = std::min(w.capacity, end - base); init.n = init.n_new; init.issued = base + init.n_new;
+            CU(cudaMemcpyAsync(w.ctl, &init, sizeof(Ctl), cudaMemcpyHostToDevice, st[h]));
+            bound[h] = init.n; live[h] = true;
+        }
+        // The host runs one iteration ahead of the device: after enqueueing iteration i of both wavefronts it waits for their
+        // snapshots taken after iteration i-1 (normally long complete), which bound the grids of iteration i+1 and tell when a
+        // wavefront has drained; a drained wavefront is no longer enqueued.
+        for (uint32_t iter = 0; live[0] || live[1]; ++iter) {
+            if (c->abort_flag.load()) { cudaStreamSynchronize(st[1]); cudaStreamSynchronize(st[0]); c->abort_flag.store(0); return fail(c, TGB_ERR_ABORTED, "render aborted"); }
             const int slot = int(iter & 3u);
-            enqueue_iteration(c, bi, cur, bound, slot, launches);
-            cur ^= 1;
-            CU(cudaMemcpyAsync(&c->h_ctl[slot], c->ctl, sizeof(Ctl), cudaMemcpyDeviceToHost, c->stream));
-            CU(cudaEventRecord(c->ev_ring[slot], c->stream));
-            if (iter == 0) { bound = std::min(c->capacity, total); continue; }      // nothing known yet about iteration 1
-            const int p = int((iter - 1) & 3u);
-            CU(cudaEventSynchronize(c->ev_ring[p]));
-            const Ctl S = c->h_ctl[p];                        // state after iteration iter-1 = the sizes of iteration iter
-            if (c->profiling) {
-                for (int k = 0; k < 7; ++k) { float ms = 0.0f; cudaEventElapsedTime(&ms, c->ev_k[p][k], c->ev_k[p][k + 1]); kms[k] += ms; }
-                trace_launches++; shadow_launches++;           // one k_trace and one k_shadow_bvh per timed iteration
+            for (int h = 0; h < 2; ++h) {
+                if (!live[h]) continue;
+                Wavefront &w = c->wf[h];
+                enqueue_iteration(c, w, st[h], bi, cur[h], bound[h], slot, launches);
+                cur[h] ^= 1;
+                CU(cudaMemcpyAsync(&w.h_ctl[slot], w.ctl, sizeof(Ctl), cudaMemcpyDeviceToHost, st[h]));
+                CU(cudaEventRecord(w.ev_ring[slot], st[h]));
             }
-            if (trace_bounces) fprintf(stderr, "after iter %u: next n %u (survivors %u, new %u, to traverse %u) issued %u/%u\n", iter - 1, S.n, S.n_surv, S.n_new, S.n_sorted, S.issued, S.total);
-            if (S.n == 0) { traversed += S.traversed; shadow_traversed += S.shadow_traversed; iterations += S.iterations; break; }   // iteration `iter`, already queued, is empty
-            // n(iter+1) <= n(iter) + the camera paths not yet issued after iteration iter's refill
-            bound = uint32_t(std::min<uint64_t>(c->capacity, uint64_t(S.n) + (S.total - S.issued)));
+            if (iter == 0) continue;                          // nothing known yet about iteration 1: its bound stays the first one
+            const int p = int((iter - 1) & 3u);
+            for (int h = 0; h < 2; ++h) {
+                if (!live[h]) continue;
+                Wavefront &w = c->wf[h];
+                CU(cudaEventSynchronize(w.ev_ring[p]));
+                const Ctl S = w.h_ctl[p];                     // state after iteration iter-1 = the sizes of iteration iter
+                if (c->profiling) {
+                    for (int k = 0; k < 7; ++k) { float ms = 0.0f; cudaEventElapsedTime(&ms, w.ev_k[p][k], w.ev_k[p][k + 1]); kms[k] += ms; }
+                    trace_launches++; shadow_launches++;       // one k_trace and one k_shadow_bvh per timed iteration
+                }
+                if (trace_bounces) fprintf(stderr, "wavefront %d after iter %u: next n %u (survivors %u, new %u, to traverse %u) issued %u/%u\n", h, iter - 1, S.n, S.n_surv, S.n_new, S.n_sorted, S.issued, S.total);
+                if (S.n == 0) { traversed += S.traversed; shadow_traversed += S.shadow_traversed; iterations += S.iterations; live[h] = false; continue; }   // iteration `iter`, already queued, is empty
+                // n(iter+1) <= n(iter) + the camera paths not yet issued after iteration iter's refill
+                bound[h] = uint32_t(std::min<uint64_t>(w.capacity, uint64_t(S.n) + (S.total - S.issued)));
+            }
             if (iter > (1u << 24)) return fail(c, TGB_ERR_INVALID, "wavefront loop did not terminate");
         }
-        k_resolve<<<blocks(c->n_pix, 256), 256, 0, c->stream>>>(c->sr.R, bi, ns, c->fb, c->fb_count); launches++;
+        // join: k_resolve, and whatever the caller queues on its stream after this call, wait for wavefront 1
+        CU(cudaEventRecord(c->ev_join, st[1]));
+        CU(cudaStreamWaitEvent(st[0], c->ev_join, 0));
+        k_resolve<<<blocks(c->n_pix, 256), 256, 0, st[0]>>>(c->R, bi, ns, c->fb, c->fb_count); launches++;
     }
     CU(cudaEventRecord(c->ev1, c->stream));
     CU(cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(Counters), cudaMemcpyDeviceToHost, c->stream));
@@ -1076,14 +1116,18 @@ void tgb200_destroy(tgb_ctx *c) {
     }
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
+    if (c->stream1) cudaStreamSynchronize(c->stream1);
     for (void *p : c->allocs) cudaFree(p);
-    if (c->sr.R) cudaFree(c->sr.R);
-    if (c->h_ctl) cudaFreeHost(c->h_ctl);
+    if (c->R) cudaFree(c->R);
     if (c->h_ctr) cudaFreeHost(c->h_ctr);
     if (c->h_fb) cudaFreeHost(c->h_fb);
     if (c->h_fb_count) cudaFreeHost(c->h_fb_count);
-    for (cudaEvent_t e : {c->ev0, c->ev1}) if (e) cudaEventDestroy(e);
-    for (int k = 0; k < 4; ++k) { if (c->ev_ring[k]) cudaEventDestroy(c->ev_ring[k]); for (cudaEvent_t e : c->ev_k[k]) if (e) cudaEventDestroy(e); }
+    for (cudaEvent_t e : {c->ev0, c->ev1, c->ev_fork, c->ev_join}) if (e) cudaEventDestroy(e);
+    for (Wavefront &w : c->wf) {
+        if (w.h_ctl) cudaFreeHost(w.h_ctl);
+        for (int k = 0; k < 4; ++k) { if (w.ev_ring[k]) cudaEventDestroy(w.ev_ring[k]); for (cudaEvent_t e : w.ev_k[k]) if (e) cudaEventDestroy(e); }
+    }
+    if (c->stream1) cudaStreamDestroy(c->stream1);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;
 }
@@ -1153,19 +1197,23 @@ static int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
     int rc = TGB_OK;
     do {
         if (cudaSetDevice(dev) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", dev); break; }
-        if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaStreamCreate failed"); break; }
+        if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaStreamCreateWithFlags(&c->stream1, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaStreamCreate failed"); break; }
         c->stream = c->own_stream;
         for (cudaEvent_t *e : {&c->ev0, &c->ev1}) cudaEventCreate(e);
-        for (int k = 0; k < 4; ++k) {
-            cudaEventCreateWithFlags(&c->ev_ring[k], cudaEventDisableTiming);
-            for (cudaEvent_t &e : c->ev_k[k]) cudaEventCreate(&e);
-        }
+        for (cudaEvent_t *e : {&c->ev_fork, &c->ev_join}) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
+        for (Wavefront &w : c->wf)
+            for (int k = 0; k < 4; ++k) {
+                cudaEventCreateWithFlags(&w.ev_ring[k], cudaEventDisableTiming);
+                for (cudaEvent_t &e : w.ev_k[k]) cudaEventCreate(&e);
+            }
         if ((rc = upload_scene(c, d))) break;
-        uint32_t cap = d->settings.max_paths_in_flight ? d->settings.max_paths_in_flight : (1u << 22);
+        // default: 2 x 4 Mi paths in flight (H100, C1: 2 x 2 Mi measured 3 % slower)
+        uint32_t cap = d->settings.max_paths_in_flight ? d->settings.max_paths_in_flight : (1u << 23);
         cap = std::max(cap, 1024u);
         if ((rc = alloc_wavefront(c, cap))) break;
-        {   // persistent traversal grid = twice what is resident at once (blocks per SM x SMs, smaller of the two kernels): the
-            // second wave evens out the end of a launch
+        {   // persistent traversal grid of one wavefront: what is resident at once (blocks per SM x SMs, smaller of the two
+            // kernels), or TGB_TRAVERSAL_BLOCKS per SM.  H100, C1: 6 (resident) > 4 > 12 (twice resident) > 3 blocks per SM.
             int sms = 0, b1 = 0, b2 = 0;
             cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
             cudaError_t e = cudaSuccess;
@@ -1175,8 +1223,8 @@ static int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
             if (c->has_curves) { prep(k_trace<true>, &b1); prep(c->mesh_lights ? k_shadow_bvh<true, true> : k_shadow_bvh<true, false>, &b2); }
             else { prep(k_trace<false>, &b1); prep(c->mesh_lights ? k_shadow_bvh<false, true> : k_shadow_bvh<false, false>, &b2); }
             if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
-            const char *mult = getenv("TGB_PERSIST_MULT");
-            c->persist_blocks = uint32_t(sms*std::min(b1, b2))*uint32_t(mult ? std::max(1, atoi(mult)) : 2);
+            const char *per_sm = getenv("TGB_TRAVERSAL_BLOCKS");
+            c->persist_blocks = uint32_t(sms)*uint32_t(per_sm ? std::max(1, atoi(per_sm)) : std::min(b1, b2));
         }
     } while (0);
     if (rc) { g_create_error = c->error; tgb200_destroy(c); return rc; }
@@ -1279,11 +1327,12 @@ static cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t
     }
     if (e == cudaSuccess && c->sc.n_nodes) {
         // the renderer's own persistent kernel body (lane refill)
-        e = cudaMemsetAsync(&c->ctl->cursor_trace, 0, sizeof(uint32_t), c->stream);
+        uint32_t *cursor = &c->wf[0].ctl->cursor_trace;
+        e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), c->stream);
         uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
         if (e == cudaSuccess) {
-            if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
-            else k_hook_persist<false><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, &c->ctl->cursor_trace);
+            if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, cursor);
+            else k_hook_persist<false><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, cursor);
         }
         c->stats.kernel_launches++;
     }
@@ -1545,7 +1594,7 @@ int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
     if ((rc = render_device(c, 0, 0, true, uint32_t(total)))) return rc;
     BatchInfo bi; bi.pix_id = c->pix_id; bi.pix_seed = c->pix_seed; bi.n_pix = c->n_pix; bi.spp_begin = 0;
     bi.pix_first = c->pix_first; bi.pix_base = c->pix_base; bi.pix_bits = pix_bits;
-    k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->sr.R, bi, c->pix_slot, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
+    k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R, bi, c->pix_slot, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
     c->stats.kernel_launches++;
     CU(cudaMemcpyAsync(records, c->rec_dev, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
@@ -1923,28 +1972,29 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
     if (e == cudaSuccess) e = b.alloc(&ctl_saved, 1);
     if (e == cudaSuccess) e = b.alloc(&ctr_saved, 1);
     // the probe's queries must not show in the context's control block or in the next render's statistics
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, c->ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+    const Wavefront &w = c->wf[0];
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, w.ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
     if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
     const bool saved = e == cudaSuccess;
     const DScene &sc = c->sc; const bool curves = c->has_curves; cudaStream_t st = c->stream;
-    // one scratch slot per query: chunks of the context's capacity
-    for (uint32_t off = 0; off < n && e == cudaSuccess; off += c->capacity) {
-        const uint32_t m = std::min(c->capacity, n - off);
+    // one scratch slot per query: chunks of wavefront 0's capacity
+    for (uint32_t off = 0; off < n && e == cudaSuccess; off += w.capacity) {
+        const uint32_t m = std::min(w.capacity, n - off);
         // shadow_count, shadow_count2, cursor_trace, cursor_shadow, shadow_count_closest, cursor_closest
-        e = cudaMemsetAsync(&c->ctl->shadow_count, 0, 6*sizeof(uint32_t), st);
+        e = cudaMemsetAsync(&w.ctl->shadow_count, 0, 6*sizeof(uint32_t), st);
         if (e != cudaSuccess) break;
-        k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, c->sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
-                                                            c->squeue, c->ctl, m);
-        if (curves) k_shadow_prep<true><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
-        else k_shadow_prep<false><<<blocks(m, 256), 256, 0, st>>>(sc, c->sr, c->squeue, c->ctl, c->squeue2, c->squeue_cl, c->ctr);
-        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(c->squeue2, c->squeue_cl, c->ctl, dout + 8*size_t(off));
-        if (sc.n_nodes) launch_shadow_bvh(c, std::min(blocks(m, kTraceBlock), c->persist_blocks));
-        k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(c->sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
+        k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, w.sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
+                                                            w.squeue, w.ctl, m);
+        if (curves) k_shadow_prep<true><<<blocks(m, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+        else k_shadow_prep<false><<<blocks(m, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(w.squeue2, w.squeue_cl, w.ctl, dout + 8*size_t(off));
+        if (sc.n_nodes) launch_shadow_bvh(c, w, st, std::min(blocks(m, kTraceBlock), c->persist_blocks));
+        k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(w.sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
         e = cudaGetLastError();
     }
     // restored also when a launch failed (the copies are queued after whatever was queued)
     if (saved) {
-        const cudaError_t r1 = cudaMemcpyAsync(c->ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, st);
+        const cudaError_t r1 = cudaMemcpyAsync(w.ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, st);
         const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, st);
         if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
     }
