@@ -277,14 +277,16 @@ int  tgb200_bvh_selftest(const float *tri_verts, uint32_t n, uint32_t *n_nodes, 
 /* Host-only: the hair BCSDF tables tgb200_create precomputes for one material (HairBcsdf.cpp:318-446): tables = 3 lobes
  * (R, TT, TRT) x 64 x 64 x RGB, sums = 3 x 64 row sums of the sampling weights, v = the three longitudinal variances. */
 int  tgb200_hair_selftest(float roughness, float scale_angle_deg, const float *sigma_a, float *tables, float *sums, float *v);
-/* Host-only check of the quantised device BVH (QNode4, 8-bit child boxes): walks it on the host
- * with the kernels' node arithmetic for n_rays rays (8 floats each: o, d, tmin, tmax) and compares the closest t with brute
- * force over all triangles, bit for bit.  *mismatches = rays that differ (must be 0).                                   */
+/* Host-only check of the quantised device BVH (QNode4, 8-bit child boxes): builds the tree tgb200_create builds for a scene of
+ * n triangles (the rays' origins take the camera's part in the box padding), walks it on the host with the kernels' node
+ * arithmetic and triangle test on the records tgb200_create uploads for n_rays rays (8 floats each: o, d, tmin, tmax) and
+ * compares the closest t with brute force over all triangles, bit for bit.  *mismatches = rays that differ (must be 0).  */
 int  tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays,
                           uint32_t *mismatches, uint32_t *n_nodes, uint64_t *node_visits);
-/* Host-only count of the any-hit shadow walk (no GPU): builds n triangles' tree as tgb200_create does, then walks n_queries
- * occlusion queries (8 floats each: o, d, tnear, t_light) both as a sorted walk from the root and as the unsorted walk from the
- * top-level cut boxes the segment enters.  out = 10 uint32 per query: cut mask, deepest stack of the cut walk, then per walk
+/* Host-only count of the any-hit shadow walk (no GPU): builds the tree, top-level cut and records tgb200_create builds for a
+ * scene of n triangles seen from camera_pos, then walks n_queries occlusion queries (8 floats each: o, d, tnear, t_light)
+ * both as a sorted walk from the root and as the unsorted walk from the top-level cut boxes the segment enters.
+ * out = 10 uint32 per query: cut mask, deepest stack of the cut walk, then per walk
  * (root, cut): occluded, node visits, leaf trips, triangle tests.  *stack_need = the traversal stack bound tgb200_create checks;
  * TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the traversal's own stack).                                           */
 int  tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *camera_pos, const float *queries, uint32_t n_queries,

@@ -45,6 +45,22 @@ def test_stack_bound_rejects_a_tree_deeper_than_the_stack(scratch):
     assert rc == abi.TGB_OK
 
 
+def test_walk_count_follows_the_build_switches(scratch, monkeypatch):
+    # TGB_TRI_LEAF changes the tree tgb200_create builds, so it must change the tree the host count walks
+    fs, (tris, q) = _room(scratch)
+    monkeypatch.delenv("TGB_TRI_LEAF", raising=False)
+    totals = []
+    for leaf in (None, "2"):
+        if leaf:
+            monkeypatch.setenv("TGB_TRI_LEAF", leaf)
+        rc, _, out = swc.walk_counts(tris, F(fs.camera.pos), q)
+        agree, _ = swc.summary(out)
+        assert rc == abi.TGB_OK and agree
+        totals.append(out[:, [3, 5, 7, 9]].astype(np.int64).sum(0))   # node visits, triangle tests: root walk, cut walk
+    print("node visits / triangle tests (root, cut): leaf cap 4 %s, leaf cap 2 %s" % tuple(totals))
+    assert not np.array_equal(totals[0], totals[1])
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["cube_city", "many_lights", "hair"])
 def test_cut_entry_does_not_change_shadow_queries(name, scratch, monkeypatch):

@@ -99,6 +99,12 @@ struct Builder {
 inline float pad_down(float v) { return std::nextafter(std::nextafter(v, -std::numeric_limits<float>::infinity()), -std::numeric_limits<float>::infinity()); }
 inline float pad_up(float v) { return std::nextafter(std::nextafter(v, std::numeric_limits<float>::infinity()), std::numeric_limits<float>::infinity()); }
 
+Node4 empty_node() {
+    Node4 nd; std::memset(&nd, 0, sizeof(nd));
+    for (int k = 0; k < 4; ++k) nd.link[k] = kEmptyLink;
+    return nd;
+}
+
 }  // namespace
 
 static void build_from_boxes(std::vector<Box> &tb, std::vector<float> &cent, uint32_t n, Bvh4 &out, int threads, uint32_t max_leaf = 4, float isect_cost = 1.0f);
@@ -147,11 +153,6 @@ static void build_from_boxes(std::vector<Box> &tb, std::vector<float> &cent, uin
     auto set_child = [](Node4 &nd, int k, const Box &b, int32_t link) {
         nd.f[k] = b.lo[0]; nd.f[4 + k] = b.hi[0]; nd.f[8 + k] = b.lo[1]; nd.f[12 + k] = b.hi[1]; nd.f[16 + k] = b.lo[2]; nd.f[20 + k] = b.hi[2];
         nd.link[k] = link;
-    };
-    auto empty_node = []() {
-        Node4 nd; std::memset(&nd, 0, sizeof(nd));
-        for (int k = 0; k < 4; ++k) nd.link[k] = kEmptyLink;
-        return nd;
     };
     if (rt.left < 0) {                       // the whole scene fits one leaf
         Node4 nd = empty_node();
@@ -308,6 +309,98 @@ void qnode_slab_host(const QNode4 &nd, const float o[3], const float inv_d[3], f
         }
         t_out[k] = (tn <= tf && nd.link[k] != kEmptyLink) ? tn : std::numeric_limits<float>::infinity();
     }
+}
+
+// ---- the scene's tree -------------------------------------------------------------------------------------------
+void build_scene_bvh(const SceneBvhInput &in, const BvhOptions &opt, SceneBvh &out) {
+    const uint32_t n_tris = in.n_tris, n_curve = in.n_curve, analytic_base = n_tris + n_curve + 1;
+    // Box padding that covers the rounding of the fused slab test t = fma(lo, 1/d, -(o/d)): spatial error
+    // <= (2|o| + |lo|) * 2^-24, so 1e-6 x the largest coordinate magnitude in play (scene or camera) is ample.
+    float extent = in.extent;
+    for (uint32_t i = 0; i < n_tris; ++i) {
+        const BuildTri &t = in.tris[i];
+        for (int k = 0; k < 3; ++k) extent = std::max(extent, std::max(std::fabs(t.v0[k]), std::max(std::fabs(t.v1[k]), std::fabs(t.v2[k]))));
+    }
+    for (uint32_t i = 0; i < n_curve; ++i)
+        for (const float *q = in.curve_recs[i].f; q < in.curve_recs[i].f + 12; q += 4)
+            extent = std::max(extent, std::max(std::fabs(q[0]), std::max(std::fabs(q[1]), std::fabs(q[2]))) + q[3]);
+    Bvh4 &bvh = out.tree;                               // the triangle tree, then the merged one
+    Bvh4 cb, ab;                                        // curve pieces, analytic primitives
+    build_bvh4(in.tris, n_tris, bvh, 0, 1e-6f*extent, opt.tri_leaf, opt.tri_cost);
+    if (n_curve) build_bvh4_boxes(in.curve_boxes, n_curve, cb, 0, 1e-6f*extent, opt.curve_leaf, opt.curve_cost);
+    if (in.n_analytic) {
+        std::vector<BuildBox> aboxes(in.n_analytic);
+        for (uint32_t k = 0; k < in.n_analytic; ++k) {
+            const Aabb &b = in.analytic[k];
+            // the primitives' own tests work on a point o + d*t computed in fp32: pad by the rounding of that point as well.
+            // Their unpadded bounds raise the extent for this tree only (the two above are already built).
+            for (int a = 0; a < 3; ++a) {
+                const float pad = 4e-6f*std::max(std::fabs(b.lo[a]), std::fabs(b.hi[a]));
+                aboxes[k].lo[a] = b.lo[a] - pad; aboxes[k].hi[a] = b.hi[a] + pad; aboxes[k].centroid[a] = 0.5f*(b.lo[a] + b.hi[a]);
+                extent = std::max(extent, std::max(std::fabs(b.lo[a]), std::fabs(b.hi[a])));
+            }
+        }
+        build_bvh4_boxes(aboxes.data(), in.n_analytic, ab, 0, 2e-6f*extent, 2, 2.0f);
+    }
+    out.analytic_order = ab.order;
+    {
+        // the trees that exist hang under one new root (a single tree keeps its own root), so ONE traversal answers
+        // TraceableScene::intersect
+        struct Sub { const Bvh4 *b; uint32_t pos_base; bool flag; };
+        std::vector<Sub> subs;
+        if (!bvh.nodes.empty()) subs.push_back({&bvh, 0u, false});
+        if (!cb.nodes.empty()) subs.push_back({&cb, n_tris, true});
+        if (!ab.nodes.empty()) subs.push_back({&ab, analytic_base, true});
+        const bool rooted = subs.size() > 1;
+        if (rooted || (subs.size() == 1 && subs[0].b != &bvh)) {
+            size_t total = rooted ? 1 : 0;
+            for (const Sub &sb : subs) total += sb.b->nodes.size();
+            std::vector<Node4> merged(total);
+            Node4 root = empty_node();
+            float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
+            uint32_t depth = 0; double sah = 0.0;
+            int32_t base = rooted ? 1 : 0;
+            for (size_t t = 0; t < subs.size(); ++t) {
+                const Sub &sb = subs[t];
+                for (size_t k = 0; k < sb.b->nodes.size(); ++k) {
+                    Node4 nd = sb.b->nodes[k];
+                    for (int j = 0; j < 4; ++j) {
+                        if (nd.link[j] >= 0) nd.link[j] += base;
+                        else if (nd.link[j] != kEmptyLink) { const int32_t code = ~nd.link[j]; nd.link[j] = ~int32_t((((code >> 3) + int32_t(sb.pos_base)) << 3) | (sb.flag ? 4 : 0) | (code & 3)); }
+                    }
+                    merged[size_t(base) + k] = nd;
+                }
+                for (int a = 0; a < 3; ++a) {
+                    root.f[8*a + t] = sb.b->lo[a]; root.f[8*a + 4 + t] = sb.b->hi[a];
+                    lo[a] = std::min(lo[a], sb.b->lo[a]); hi[a] = std::max(hi[a], sb.b->hi[a]);
+                }
+                root.link[t] = base;
+                depth = std::max(depth, sb.b->max_depth); sah += sb.b->sah_cost;
+                base += int32_t(sb.b->nodes.size());
+            }
+            if (rooted) { merged[0] = root; depth += 1; }
+            std::vector<uint32_t> order = bvh.order;
+            for (uint32_t k : cb.order) order.push_back(n_tris + k);
+            bvh.nodes.swap(merged); bvh.order.swap(order);
+            bvh.max_depth = depth; bvh.sah_cost = sah;
+            for (int a = 0; a < 3; ++a) { bvh.lo[a] = lo[a]; bvh.hi[a] = hi[a]; }
+        }
+    }
+    out.cut = top_level_cut(bvh, opt.max_cut);
+    out.stack_need = traversal_stack_need(bvh, out.cut);
+    out.isect.assign(size_t(n_tris) + n_curve + 1, IsectRecord{});
+    for (size_t k = n_tris; k < bvh.order.size(); ++k) out.isect[k] = in.curve_recs[bvh.order[k] - n_tris];
+    for (size_t k = 0; k < n_tris; ++k) {
+        const BuildTri &t = in.tris[bvh.order[k]];
+        float *r = out.isect[k].f;                      // v0, e1, e2, then Ng = cross(e1, e2)
+        for (int a = 0; a < 3; ++a) { r[a] = t.v0[a]; r[3 + a] = t.v0[a] - t.v1[a]; r[6 + a] = t.v2[a] - t.v0[a]; }
+        r[9] = r[4]*r[8] - r[5]*r[7]; r[10] = r[5]*r[6] - r[3]*r[8]; r[11] = r[3]*r[7] - r[4]*r[6];
+    }
+    // empty child slots link to a one-primitive leaf holding the all-zero record
+    quantize_bvh4(bvh, out.qtree, ~int32_t((n_tris + n_curve) << 3));
+    std::vector<int32_t> new_index(out.qtree.old_index.size());
+    for (size_t i = 0; i < new_index.size(); ++i) new_index[size_t(out.qtree.old_index[i])] = int32_t(i);
+    for (CutBox &b : out.cut) if (b.link >= 0) b.link = new_index[size_t(b.link)];
 }
 
 }  // namespace tgb

@@ -87,4 +87,49 @@ void build_bvh4(const BuildTri *tris, uint32_t n, Bvh4 &out, int threads = 0, fl
 void build_bvh4_boxes(const BuildBox *boxes, uint32_t n, Bvh4 &out, int threads = 0, float abs_pad = 0.0f,
                       uint32_t max_leaf = 4, float isect_cost = 1.0f);
 
+// ---- the scene's tree, as tgb200_create builds and uploads it ------------------------------------------------------
+// Build switches (environment overrides: bvh_options in tgb200_api.cu).
+struct BvhOptions {
+    // SAH leaf cap and intersection cost of the triangle tree: chosen on C1 on the previous GPU (B200).  On an H100 (C1, 400 W
+    // limit) cost 1 or leaf cap 2 measured ~1 % faster and cost 2 ~2 % slower; the default is kept, as a different tree changes
+    // which of two equally distant hits wins.
+    uint32_t tri_leaf = 4; float tri_cost = 0.5f;
+    // a segment test (3 projections + up to 32 half-cylinder pieces) costs far more than a triangle test: small leaves (the
+    // reference's BinaryBvh also keeps <= 2 segments per leaf, Curves.cpp:613)
+    uint32_t curve_leaf = 2; float curve_cost = 4.0f;
+    size_t max_cut = 16;            // boxes of the top-level cut: fewer = cheaper pre-test in k_accum / k_shadow_prep, looser cut
+};
+
+struct Aabb { float lo[3], hi[3]; };
+
+// One 48-byte intersection record per leaf position, as the kernels read it (3 x float4).  Triangle (Embree TriangleM,
+// kernels/geometry/triangle.h:54): v0, e1 = v0 - v1, e2 = v2 - v0, Ng = cross(e1, e2).  Curve piece: its segment's three nodes
+// (x, y, z, width).
+struct alignas(16) IsectRecord { float f[12]; };
+
+struct SceneBvhInput {
+    const BuildTri *tris = nullptr; uint32_t n_tris = 0;
+    // curve pieces: bounds and intersection record of each
+    const BuildBox *curve_boxes = nullptr; const IsectRecord *curve_recs = nullptr; uint32_t n_curve = 0;
+    // analytic primitives that become leaves (quads / cubes): unpadded world bounds; n_analytic = 0 keeps them out of the tree
+    const Aabb *analytic = nullptr; uint32_t n_analytic = 0;
+    // largest coordinate magnitude in play besides the primitives' (the camera position): seeds the padding extent
+    float extent = 0.0f;
+};
+
+// Leaf positions: [0, n_tris) triangles, [n_tris, n_tris + n_curve) curve pieces, one all-zero record (the target of empty
+// child slots; every primitive test rejects it), then the analytic primitives from isect.size() on.  Leaves of the last two
+// kinds carry bit 2 of the leaf code.
+struct SceneBvh {
+    Bvh4 tree;                           // every tree under one root; tree.order: leaf position -> triangle, then n_tris + curve piece
+    QBvh4 qtree;                         // its device layout
+    std::vector<uint32_t> analytic_order;   // analytic leaf position - isect.size() -> analytic input index
+    std::vector<IsectRecord> isect;      // tris + curve pieces + 1, in leaf order
+    std::vector<CutBox> cut;             // top-level cut, link = QNode4 index (or leaf code) below each box
+    uint32_t stack_need = 0;             // traversal_stack_need of the tree and its cut
+};
+// One tree for the triangles, one for the curve pieces and one for the analytic primitives (those that exist), under a joint
+// root when there are several, then the cut, the device layout and the records.
+void build_scene_bvh(const SceneBvhInput &in, const BvhOptions &opt, SceneBvh &out);
+
 }  // namespace tgb

@@ -255,6 +255,27 @@ void build_spherical_distribution(const tgb_texture &t, HostTex &ht) {
     ht.has_dist = true;
 }
 
+// The BVH build switches: BvhOptions' defaults, overridden from the environment (DESIGN.md section 6).  tgb200_create and the
+// host-only BVH checks read them alike, so the checks walk the tree tgb200_create builds.
+BvhOptions bvh_options() {
+    BvhOptions o;
+    if (const char *e = getenv("TGB_TRI_LEAF")) o.tri_leaf = uint32_t(atoi(e));
+    if (const char *e = getenv("TGB_TRI_COST")) o.tri_cost = float(atof(e));
+    if (const char *e = getenv("TGB_CURVE_LEAF")) o.curve_leaf = uint32_t(atoi(e));
+    if (const char *e = getenv("TGB_CURVE_COST")) o.curve_cost = float(atof(e));
+    if (const char *e = getenv("TGB_CUT_BOXES")) o.max_cut = size_t(std::min(16, std::max(4, atoi(e))));
+    return o;
+}
+
+// World bounds of a quad's four corners or a cube's eight
+Aabb analytic_bounds(const DPrim &p) {
+    Aabb b = {{INFINITY, INFINITY, INFINITY}, {-INFINITY, -INFINITY, -INFINITY}};
+    auto grow = [&](V3 q) { float v[3] = {q.x, q.y, q.z}; for (int a = 0; a < 3; ++a) { b.lo[a] = std::min(b.lo[a], v[a]); b.hi[a] = std::max(b.hi[a], v[a]); } };
+    if (p.type == TGB_PRIM_QUAD) { grow(p.base); grow(p.base + p.edge0); grow(p.base + p.edge1); grow(p.base + p.edge0 + p.edge1); }
+    else for (int j = 0; j < 8; ++j) grow(p.pos + m3mul(p.rot, v3((j & 1 ? p.scale.x : -p.scale.x), (j & 2 ? p.scale.y : -p.scale.y), (j & 4 ? p.scale.z : -p.scale.z))));
+    return b;
+}
+
 int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
     const tgb_camera &cam = d->camera;
     DScene &sc = c->sc;
@@ -335,7 +356,7 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
     std::vector<DPrim> prims(d->n_primitives);
     std::vector<int> lights, inf_lights, analytic;
     std::vector<BuildTri> btris; std::vector<uint32_t> tri_prim; std::vector<float4> tri_shade;
-    std::vector<BuildBox> cboxes; std::vector<float4> crecs; std::vector<uint32_t> cseg_prim;   // curve BVH primitives (kCurvePieces per segment) of all primitives
+    std::vector<BuildBox> cboxes; std::vector<IsectRecord> crecs; std::vector<uint32_t> cseg_prim;   // curve BVH primitives (kCurvePieces per segment) of all primitives
     int lightCount = 0;
     for (uint32_t i = 0; i < d->n_primitives; ++i) {
         const tgb_primitive &p = d->primitives[i]; DPrim &o = prims[i];
@@ -459,8 +480,8 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
                         bb.centroid[a] = 0.5f*(lo + hi);
                     }
                     cboxes.push_back(bb); cseg_prim.push_back(i);
-                    crecs.push_back(make_float4(n0[0], n0[1], n0[2], n0[3])); crecs.push_back(make_float4(n1[0], n1[1], n1[2], n1[3]));
-                    crecs.push_back(make_float4(n2[0], n2[1], n2[2], n2[3]));
+                    IsectRecord rec; std::memcpy(rec.f, n0, sizeof(rec.f));        // n0, n1, n2
+                    crecs.push_back(rec);
                 }
             }
             break; }
@@ -501,162 +522,51 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         dtex[i] = tex[i].d;
     }
 
-    // ---- BVH over every mesh triangle
-    Bvh4 bvh;
-    // Box padding that covers the rounding of the fused slab test t = fma(lo, 1/d, -(o/d)): spatial error
-    // <= (2|o| + |lo|) * 2^-24, so 1e-6 x the largest coordinate magnitude in play (scene or camera) is ample.
-    float extent = std::max(std::max(std::fabs(sc.cam.pos.x), std::fabs(sc.cam.pos.y)), std::fabs(sc.cam.pos.z));
-    for (const BuildTri &t : btris) for (int k = 0; k < 3; ++k)
-        extent = std::max(extent, std::max(std::fabs(t.v0[k]), std::max(std::fabs(t.v1[k]), std::fabs(t.v2[k]))));
-    for (const float4 &q : crecs) extent = std::max(extent, std::max(std::fabs(q.x), std::max(std::fabs(q.y), std::fabs(q.z))) + q.w);
-    {
-        // SAH intersection cost and leaf cap: chosen on C1 on the previous GPU (B200).  On an H100 (C1, 400 W limit) cost 1 or
-        // leaf cap 2 measured ~1 % faster and cost 2 ~2 % slower; the default is kept, as a different tree changes which of
-        // two equally distant hits wins.
-        uint32_t tri_leaf = 4; float tri_cost = 0.5f;
-        if (const char *e = getenv("TGB_TRI_LEAF")) tri_leaf = uint32_t(atoi(e));
-        if (const char *e = getenv("TGB_TRI_COST")) tri_cost = float(atof(e));
-        build_bvh4(btris.data(), uint32_t(btris.size()), bvh, 0, 1e-6f*extent, tri_leaf, tri_cost);
-    }
-    const uint32_t n_tris_total = uint32_t(btris.size()), n_segs_total = uint32_t(cboxes.size());
-    // Leaf positions: [0, n_tris) triangles, [n_tris, n_tris + n_segs) curve segments, one all-zero record (the target of empty
-    // child slots), then -- only when they are many -- the analytic primitives.  Leaves of the last two kinds carry bit 2.
+    // ---- BVH over every mesh triangle, curve piece and -- only when they are many -- analytic primitive.
     // Analytic quads/cubes are few in most scenes and are then tested coherently by the kernel that creates a ray; from
     // TGB_ANALYTIC_BVH_MIN (24) primitives on they get a third SAH tree instead (the reference keeps them in Embree's top-level
     // user-geometry BVH, renderer/TraceableScene.hpp:112-134), so a ray's cost no longer grows with their number.
     size_t analytic_bvh_min = 24;
     if (const char *e = getenv("TGB_ANALYTIC_BVH_MIN")) analytic_bvh_min = size_t(std::max(1, atoi(e)));
     const bool analytic_in_bvh = analytic.size() >= analytic_bvh_min;
-    const uint32_t analytic_base = n_tris_total + n_segs_total + 1;
-    Bvh4 cb, ab;
-    if (n_segs_total) {
-        // a segment test (3 projections + up to 32 half-cylinder pieces) costs far more than a triangle test: small leaves
-        // (the reference's BinaryBvh also keeps <= 2 segments per leaf, Curves.cpp:613)
-        uint32_t curve_leaf = 2; float curve_cost = 4.0f;
-        if (const char *e = getenv("TGB_CURVE_LEAF")) curve_leaf = uint32_t(atoi(e));
-        if (const char *e = getenv("TGB_CURVE_COST")) curve_cost = float(atof(e));
-        build_bvh4_boxes(cboxes.data(), n_segs_total, cb, 0, 1e-6f*extent, curve_leaf, curve_cost);
-    }
-    if (analytic_in_bvh) {
-        std::vector<BuildBox> aboxes(analytic.size());
-        for (size_t k = 0; k < analytic.size(); ++k) {
-            const DPrim &p = prims[size_t(analytic[k])];
-            float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-            auto grow = [&](V3 q) { float v[3] = {q.x, q.y, q.z}; for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], v[a]); hi[a] = std::max(hi[a], v[a]); } };
-            if (p.type == TGB_PRIM_QUAD) { grow(p.base); grow(p.base + p.edge0); grow(p.base + p.edge1); grow(p.base + p.edge0 + p.edge1); }
-            else for (int j = 0; j < 8; ++j) grow(p.pos + m3mul(p.rot, v3((j & 1 ? p.scale.x : -p.scale.x), (j & 2 ? p.scale.y : -p.scale.y), (j & 4 ? p.scale.z : -p.scale.z))));
-            // the primitives' own tests work on a point o + d*t computed in fp32: pad by the rounding of that point as well
-            for (int a = 0; a < 3; ++a) {
-                const float pad = 4e-6f*std::max(std::fabs(lo[a]), std::fabs(hi[a]));
-                aboxes[k].lo[a] = lo[a] - pad; aboxes[k].hi[a] = hi[a] + pad; aboxes[k].centroid[a] = 0.5f*(lo[a] + hi[a]);
-                extent = std::max(extent, std::max(std::fabs(lo[a]), std::fabs(hi[a])));
-            }
-        }
-        build_bvh4_boxes(aboxes.data(), uint32_t(aboxes.size()), ab, 0, 2e-6f*extent, 2, 2.0f);
-    }
-    {
-        // the trees that exist hang under one new root (a single tree keeps its own root), so ONE traversal answers
-        // TraceableScene::intersect
-        struct Sub { Bvh4 *b; uint32_t pos_base; bool flag; };
-        std::vector<Sub> subs;
-        if (!bvh.nodes.empty()) subs.push_back({&bvh, 0u, false});
-        if (!cb.nodes.empty()) subs.push_back({&cb, n_tris_total, true});
-        if (!ab.nodes.empty()) subs.push_back({&ab, analytic_base, true});
-        const bool rooted = subs.size() > 1;
-        if (rooted || (subs.size() == 1 && subs[0].b != &bvh)) {
-            size_t total = rooted ? 1 : 0;
-            for (const Sub &sb : subs) total += sb.b->nodes.size();
-            std::vector<Node4> merged(total);
-            Node4 root; std::memset(&root, 0, sizeof(root));
-            for (int j = 0; j < 4; ++j) root.link[j] = kEmptyLink;
-            float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-            uint32_t depth = 0; double sah = 0.0;
-            int32_t base = rooted ? 1 : 0;
-            for (size_t t = 0; t < subs.size(); ++t) {
-                const Sub &sb = subs[t];
-                for (size_t k = 0; k < sb.b->nodes.size(); ++k) {
-                    Node4 nd = sb.b->nodes[k];
-                    for (int j = 0; j < 4; ++j) {
-                        if (nd.link[j] >= 0) nd.link[j] += base;
-                        else if (nd.link[j] != kEmptyLink) { const int32_t code = ~nd.link[j]; nd.link[j] = ~int32_t((((code >> 3) + int32_t(sb.pos_base)) << 3) | (sb.flag ? 4 : 0) | (code & 3)); }
-                    }
-                    merged[size_t(base) + k] = nd;
-                }
-                for (int a = 0; a < 3; ++a) {
-                    root.f[8*a + t] = sb.b->lo[a]; root.f[8*a + 4 + t] = sb.b->hi[a];
-                    lo[a] = std::min(lo[a], sb.b->lo[a]); hi[a] = std::max(hi[a], sb.b->hi[a]);
-                }
-                root.link[t] = base;
-                depth = std::max(depth, sb.b->max_depth); sah += sb.b->sah_cost;
-                base += int32_t(sb.b->nodes.size());
-            }
-            if (rooted) { merged[0] = root; depth += 1; }
-            std::vector<uint32_t> order = bvh.order;
-            for (uint32_t k : cb.order) order.push_back(n_tris_total + k);
-            bvh.nodes.swap(merged); bvh.order.swap(order);
-            bvh.max_depth = depth; bvh.sah_cost = sah;
-            for (int a = 0; a < 3; ++a) { bvh.lo[a] = lo[a]; bvh.hi[a] = hi[a]; }
-        }
-        if (n_segs_total) {
-            for (uint32_t pi : cseg_prim) tri_prim.push_back(pi);
-            for (DPrim &p : prims) if (p.type == TGB_PRIM_CURVES) p.tri_first += n_tris_total;
-        }
+    std::vector<Aabb> abounds(analytic.size());
+    for (size_t k = 0; k < analytic.size(); ++k) abounds[k] = analytic_bounds(prims[size_t(analytic[k])]);
+    SceneBvhInput in;
+    in.tris = btris.data(); in.n_tris = uint32_t(btris.size());
+    in.curve_boxes = cboxes.data(); in.curve_recs = crecs.data(); in.n_curve = uint32_t(cboxes.size());
+    if (analytic_in_bvh) { in.analytic = abounds.data(); in.n_analytic = uint32_t(abounds.size()); }
+    in.extent = std::max(std::max(std::fabs(sc.cam.pos.x), std::fabs(sc.cam.pos.y)), std::fabs(sc.cam.pos.z));
+    SceneBvh sb;
+    build_scene_bvh(in, bvh_options(), sb);
+    const Bvh4 &bvh = sb.tree;
+    if (!cboxes.empty()) {
+        for (uint32_t pi : cseg_prim) tri_prim.push_back(pi);
+        for (DPrim &p : prims) if (p.type == TGB_PRIM_CURVES) p.tri_first += uint32_t(btris.size());
     }
     std::vector<int> analytic_loop = analytic;           // what the ray-creating kernels loop over
-    if (analytic_in_bvh) {                                // ... nothing: the list goes into BVH leaf order instead
-        std::vector<int> in_leaf_order(analytic.size());
-        for (size_t k = 0; k < ab.order.size(); ++k) in_leaf_order[k] = analytic[ab.order[k]];
-        analytic_loop.swap(in_leaf_order);
-    }
+    if (analytic_in_bvh)                                  // ... nothing: the list goes into BVH leaf order instead
+        for (size_t k = 0; k < sb.analytic_order.size(); ++k) analytic_loop[k] = analytic[sb.analytic_order[k]];
     {   // ray-binning grid: bounds of every finite primitive (TraceableScene::_sceneBounds, TraceableScene.hpp:104-110)
         float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-        auto grow = [&](V3 p) { float q[3] = {p.x, p.y, p.z}; for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], q[a]); hi[a] = std::max(hi[a], q[a]); } };
-        if (!bvh.nodes.empty()) { grow(f3(bvh.lo)); grow(f3(bvh.hi)); }
-        for (int pi : analytic) {
-            const DPrim &p = prims[pi];
-            if (p.type == TGB_PRIM_QUAD) { grow(p.base); grow(p.base + p.edge0); grow(p.base + p.edge1); grow(p.base + p.edge0 + p.edge1); }
-            else for (int k = 0; k < 8; ++k) grow(p.pos + m3mul(p.rot, v3((k & 1 ? p.scale.x : -p.scale.x), (k & 2 ? p.scale.y : -p.scale.y), (k & 4 ? p.scale.z : -p.scale.z))));
-        }
+        auto grow = [&](const float *p) { for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], p[a]); hi[a] = std::max(hi[a], p[a]); } };
+        if (!bvh.nodes.empty()) { grow(bvh.lo); grow(bvh.hi); }
+        for (const Aabb &b : abounds) { grow(b.lo); grow(b.hi); }
         for (int a = 0; a < 3; ++a) if (!(hi[a] > lo[a])) { lo[a] = -1.0f; hi[a] = 1.0f; }
         sc.bin_lo = v3(lo[0], lo[1], lo[2]);
         sc.bin_inv = v3(16.0f/(hi[0] - lo[0]), 16.0f/(hi[1] - lo[1]), 16.0f/(hi[2] - lo[2]));
     }
-    size_t max_cut = 16;                         // TGB_CUT_BOXES: fewer boxes = cheaper pre-test in k_accum / k_shadow_prep, looser cut
-    if (const char *e = getenv("TGB_CUT_BOXES")) max_cut = size_t(std::min(16, std::max(4, atoi(e))));
-    const std::vector<CutBox> cut = top_level_cut(bvh, max_cut);
-    sc.n_cut = int(cut.size());
-    for (int i = 0; i < sc.n_cut; ++i) for (int a = 0; a < 3; ++a) { sc.cut[2*a][i] = cut[size_t(i)].lo[a]; sc.cut[2*a + 1][i] = cut[size_t(i)].hi[a]; }
+    sc.n_cut = int(sb.cut.size());
+    for (int i = 0; i < sc.n_cut; ++i) {
+        for (int a = 0; a < 3; ++a) { sc.cut[2*a][i] = sb.cut[size_t(i)].lo[a]; sc.cut[2*a + 1][i] = sb.cut[size_t(i)].hi[a]; }
+        sc.cut_link[i] = sb.cut[size_t(i)].link;
+    }
     {
         const char *e = getenv("TGB_SHADOW_CUT_ENTRY");
         sc.cut_entry = (e && e[0] == '0') ? 0 : 1;
     }
-    const uint32_t stack_need = traversal_stack_need(bvh, cut);
-    if (stack_need > uint32_t(kStackSize)) return fail(c, TGB_ERR_UNSUPPORTED, "BVH depth %u (%u stack entries) exceeds the traversal stack", bvh.max_depth, stack_need);
+    if (sb.stack_need > uint32_t(kStackSize)) return fail(c, TGB_ERR_UNSUPPORTED, "BVH depth %u (%u stack entries) exceeds the traversal stack", bvh.max_depth, sb.stack_need);
     c->bvh_depth = bvh.max_depth; c->n_tris = uint32_t(btris.size()); c->bvh_sah = bvh.sah_cost;
-    std::vector<float4> tri_isect(3*(btris.size() + cboxes.size() + 1), make_float4(0.0f, 0.0f, 0.0f, 0.0f));   // + one all-zero record: the target of empty child slots
-    for (size_t k = btris.size(); k < bvh.order.size(); ++k) {      // curve records: the segment's three nodes + which quarter, leaf order
-        size_t seg = bvh.order[k] - btris.size();
-        for (int j = 0; j < 3; ++j) tri_isect[3*k + j] = crecs[3*seg + j];
-    }
-    for (size_t k = 0; k < btris.size(); ++k) {
-        const BuildTri &t = btris[bvh.order[k]];
-        // Embree TriangleM: v0, e1 = v0-v1, e2 = v2-v0, Ng = cross(e1, e2) (kernels/geometry/triangle.h:54)
-        V3 v0 = f3(t.v0), v1 = f3(t.v1), v2 = f3(t.v2);
-        V3 e1 = v0 - v1, e2 = v2 - v0, ng = cross(e1, e2);
-        tri_isect[3*k] = make_float4(v0.x, v0.y, v0.z, e1.x);
-        tri_isect[3*k + 1] = make_float4(e1.y, e1.z, e2.x, e2.y);
-        tri_isect[3*k + 2] = make_float4(e2.z, ng.x, ng.y, ng.z);
-    }
-    // device node layout: QNode4 (64 B, 8-bit child boxes on a per-node grid)
-    // empty child slots link to a one-triangle leaf holding the all-zero record behind the last primitive (den == 0: rejected)
-    const int32_t empty_link = ~int32_t(uint32_t(btris.size() + cboxes.size()) << 3);
-    QBvh4 qb; quantize_bvh4(bvh, qb, empty_link);
-    {
-        std::vector<int32_t> new_index(qb.old_index.size());
-        for (size_t i = 0; i < qb.old_index.size(); ++i) new_index[size_t(qb.old_index[i])] = int32_t(i);
-        for (int i = 0; i < sc.n_cut; ++i) sc.cut_link[i] = cut[size_t(i)].link >= 0 ? new_index[size_t(cut[size_t(i)].link)] : cut[size_t(i)].link;
-    }
-    c->geom_bytes = qb.nodes.size()*sizeof(QNode4) + tri_isect.size()*16 + tri_shade.size()*16 + bvh.order.size()*8;
+    c->geom_bytes = sb.qtree.nodes.size()*sizeof(QNode4) + sb.isect.size()*sizeof(IsectRecord) + tri_shade.size()*16 + bvh.order.size()*8;
 
     int rc;
     if ((rc = dev_upload(c, &sc.prims, prims))) return rc;
@@ -679,17 +589,22 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         for (size_t k = 0; k < btris.size(); ++k) std::memcpy(&shade_leaf[4*k], &tri_shade[4*size_t(bvh.order[k])], 4*sizeof(float4));
         if ((rc = dev_upload(c, &sc.tri_shade, shade_leaf))) return rc;
     }
-    if ((rc = dev_upload(c, &sc.tri_isect, tri_isect))) return rc;
+    {
+        static_assert(sizeof(IsectRecord) == 3*sizeof(float4), "intersection record layout");
+        const IsectRecord *ir = nullptr;
+        if ((rc = dev_upload(c, &ir, sb.isect))) return rc;
+        sc.tri_isect = reinterpret_cast<const float4 *>(ir);
+    }
     {
         const QNode4 *qn = nullptr;
-        if ((rc = dev_upload(c, &qn, qb.nodes))) return rc;
+        if ((rc = dev_upload(c, &qn, sb.qtree.nodes))) return rc;
         sc.qnodes = reinterpret_cast<const uint4 *>(qn); sc.qy = 0x3F80u;
     }
     std::vector<uint32_t> sobol(1024*32);
     std::memcpy(sobol.data(), tgb_sobol_blob, sobol.size()*4);
     if ((rc = dev_upload(c, &sc.sobol, sobol))) return rc;
     sc.n_prims = uint32_t(prims.size()); sc.n_lights = int(lights.size()); sc.n_inf_lights = int(inf_lights.size());
-    sc.n_analytic = analytic_in_bvh ? 0 : int(analytic.size()); sc.analytic_base = analytic_in_bvh ? int(analytic_base) : 0x7fffffff;
+    sc.n_analytic = analytic_in_bvh ? 0 : int(analytic.size()); sc.analytic_base = analytic_in_bvh ? int(sb.isect.size()) : 0x7fffffff;
     sc.n_nodes = uint32_t(bvh.nodes.size()); sc.n_tris = uint32_t(btris.size());
     sc.n_curve_segs = uint32_t(cboxes.size()); c->has_curves = !cboxes.empty();
     {
@@ -1673,10 +1588,25 @@ int tgb200_generate_work(tgb_sample_record *records, uint32_t res_x, uint32_t re
 }
 
 namespace {
-// Traversal::triangle on the host: best = t when the triangle is hit in (tnear, best)
-bool host_triangle(const BuildTri &tri, const V3 &o, const V3 &d, float tnear, float &best) {
-    V3 v0 = f3(tri.v0), v1 = f3(tri.v1), v2 = f3(tri.v2);
-    V3 e1 = v0 - v1, e2 = v2 - v0, ng = cross(e1, e2);
+// The tree tgb200_create builds for a scene of n triangles (9 floats each: v0 v1 v2) and nothing else.  extent = the largest
+// coordinate magnitude in play besides the triangles' (tgb200_create: the camera position's).
+void build_triangle_scene_bvh(const float *tri_verts, uint32_t n, float extent, SceneBvh &sb) {
+    std::vector<BuildTri> tris(n);
+    for (uint32_t i = 0; i < n; ++i) std::memcpy(&tris[i], tri_verts + 9*size_t(i), sizeof(BuildTri));
+    SceneBvhInput in;
+    in.tris = tris.data(); in.n_tris = n; in.extent = extent;
+    build_scene_bvh(in, bvh_options(), sb);
+}
+// 1/d as the kernels compute it: components no larger than 1e-30 in magnitude are replaced by +-1e-30
+void host_inv_dir(const V3 &d, float inv[3]) {
+    const float ooeps = 1e-30f;
+    inv[0] = 1.0f/(std::fabs(d.x) > ooeps ? d.x : std::copysign(ooeps, d.x));
+    inv[1] = 1.0f/(std::fabs(d.y) > ooeps ? d.y : std::copysign(ooeps, d.y));
+    inv[2] = 1.0f/(std::fabs(d.z) > ooeps ? d.z : std::copysign(ooeps, d.z));
+}
+// Traversal::triangle on the host, on the intersection record the kernels read: best = t when the triangle is hit in (tnear, best)
+bool host_triangle(const IsectRecord &rec, const V3 &o, const V3 &d, float tnear, float &best) {
+    const V3 v0 = f3(rec.f), e1 = f3(rec.f + 3), e2 = f3(rec.f + 6), ng = f3(rec.f + 9);
     V3 C = v0 - o, R = cross(d, C);
     auto edot = [](V3 a, V3 b) { return a.x*b.x + (a.y*b.y + a.z*b.z); };
     float den = edot(ng, d), absDen = std::fabs(den);
@@ -1690,21 +1620,20 @@ bool host_triangle(const BuildTri &tri, const V3 &o, const V3 &d, float tnear, f
 }
 }  // namespace
 
-// Host-only check of the quantised device BVH (no GPU needed): builds the 4-ary SAH tree over n triangles exactly as
-// tgb200_create does (same padding), quantises it (QNode4), and walks it on the HOST with the kernels' node
-// arithmetic (qnode_slab_host mirrors Traversal::visit) and their triangle test for every ray (8 floats: o, d, tmin, tmax).
-// The closest t must equal the brute-force closest t over all triangles bit for bit (ids may differ only on exact ties).
-// Returns the number of rays whose t differs in *mismatches; also verifies the link remap.
+// Host-only check of the quantised device BVH (no GPU needed): builds the tree tgb200_create builds for a scene of n triangles
+// (the rays' origins take the camera's part in the padding) and walks it on the HOST with the kernels' node arithmetic
+// (qnode_slab_host mirrors Traversal::visit) and their triangle test on the uploaded records for every ray (8 floats: o, d,
+// tmin, tmax).  The closest t must equal the brute-force closest t over all triangles bit for bit (ids may differ only on exact
+// ties).  Returns the number of rays whose t differs in *mismatches; also verifies the link remap.
 int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, uint32_t n_rays,
                          uint32_t *mismatches, uint32_t *n_nodes, uint64_t *node_visits) {
     if ((n && !tri_verts) || (n_rays && !rays) || !mismatches) return TGB_ERR_INVALID;
-    std::vector<BuildTri> tris(n);
     float extent = 0.0f;
-    for (uint32_t i = 0; i < n; ++i) { std::memcpy(&tris[i], tri_verts + 9*size_t(i), sizeof(BuildTri)); for (int k = 0; k < 9; ++k) extent = std::max(extent, std::fabs(tri_verts[9*size_t(i) + k])); }
     for (uint32_t r = 0; r < n_rays; ++r) for (int k = 0; k < 3; ++k) extent = std::max(extent, std::fabs(rays[8*size_t(r) + k]));
-    Bvh4 bvh; build_bvh4(tris.data(), n, bvh, 0, 1e-6f*extent, 4, 0.5f);
-    const int32_t empty_link = ~int32_t(n << 3);                       // a leaf past the last triangle (the walk below skips it)
-    QBvh4 qb; quantize_bvh4(bvh, qb, empty_link);
+    SceneBvh sb;
+    build_triangle_scene_bvh(tri_verts, n, extent, sb);
+    const Bvh4 &bvh = sb.tree; const QBvh4 &qb = sb.qtree;
+    const int32_t empty_link = ~int32_t(n << 3);                       // the leaf of the all-zero record behind the last triangle
     if (n_nodes) *n_nodes = uint32_t(qb.nodes.size());
     if (qb.nodes.size() != bvh.nodes.size()) return TGB_ERR_INVALID;
     for (size_t i = 0; i < qb.nodes.size(); ++i) {                      // links: same leaves, children remapped consistently
@@ -1715,19 +1644,16 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
             else if (l < 0 || size_t(l) >= qb.nodes.size() || qb.old_index[size_t(l)] != src.link[k]) return TGB_ERR_INVALID;
         }
     }
-    auto tri_test = [&](uint32_t t, const V3 &o, const V3 &d, float tnear, float &best) { host_triangle(tris[t], o, d, tnear, best); };
     uint32_t bad = 0; uint64_t visits = 0;
     std::vector<int32_t> stack;
     for (uint32_t r = 0; r < n_rays; ++r) {
         const float *ry = rays + 8*size_t(r);
         V3 o = f3(ry), d = f3(ry + 3); float tnear = ry[6], tfar = ry[7];
         float brute = tfar;
-        for (uint32_t t = 0; t < n; ++t) tri_test(t, o, d, tnear, brute);
+        for (uint32_t k = 0; k < n; ++k) host_triangle(sb.isect[k], o, d, tnear, brute);
         float best = tfar;
         if (!qb.nodes.empty()) {
-            const float ooeps = 1e-30f;
-            float inv[3] = {1.0f/(std::fabs(d.x) > ooeps ? d.x : std::copysign(ooeps, d.x)), 1.0f/(std::fabs(d.y) > ooeps ? d.y : std::copysign(ooeps, d.y)),
-                            1.0f/(std::fabs(d.z) > ooeps ? d.z : std::copysign(ooeps, d.z))};
+            float inv[3]; host_inv_dir(d, inv);
             float oo[3] = {o.x, o.y, o.z};
             stack.clear(); stack.push_back(0);
             while (!stack.empty()) {
@@ -1738,7 +1664,7 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
                     for (int k = 0; k < 4; ++k) if (t4[k] != INFINITY) stack.push_back(qb.nodes[size_t(cur)].link[k]);
                 } else {
                     int code = ~cur; uint32_t first = uint32_t(code >> 3), count = uint32_t(code & 3) + 1;
-                    for (uint32_t i = 0; i < count; ++i) if (first + i < n) tri_test(bvh.order[first + i], o, d, tnear, best);
+                    for (uint32_t i = 0; i < count; ++i) host_triangle(sb.isect[first + i], o, d, tnear, best);
                 }
             }
         }
@@ -1749,36 +1675,26 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
     return TGB_OK;
 }
 
-// Host-only count of the any-hit shadow walk's work (no GPU).  Builds the tree over n triangles as tgb200_create builds a triangle
-// scene's (padding from the larger magnitude of the triangles and the camera position), its top-level cut and QNode4 layout, and
-// walks every query (8 floats: o, d, tnear, t_light) with the kernels' node and triangle arithmetic twice: as k_shadow_bvh walked
-// any-hit queries before (children sorted near-to-far, from the root) and as it walks them now (nearest child entered, the others
-// pushed unsorted, from the cut boxes the segment enters).  A query that enters no cut box is not walked: k_shadow_prep settles it.
+// Host-only count of the any-hit shadow walk's work (no GPU).  Builds the tree, top-level cut and records tgb200_create builds for
+// a scene of n triangles seen from camera_pos, and walks every query (8 floats: o, d, tnear, t_light) with the kernels' node and
+// triangle arithmetic twice: as k_shadow_bvh walked any-hit queries before (children sorted near-to-far, from the root) and as it
+// walks them now (nearest child entered, the others pushed unsorted, from the cut boxes the segment enters).  A query that enters no cut box is not walked: k_shadow_prep settles it.
 // out = 10 uint32 per query: cut mask, deepest stack of the walk from the cut, then per walk (root, cut): occluded, node visits,
 // LEAF trips, triangle tests.  *stack_need = the bound tgb200_create checks; TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the
 // traversal's stack), before any walk.
 int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *camera_pos, const float *queries, uint32_t n_queries,
                              uint32_t stack_size, uint32_t *stack_need, uint32_t *out) {
     if (!tri_verts || n == 0 || !camera_pos || (n_queries && (!queries || !out))) return TGB_ERR_INVALID;
-    std::vector<BuildTri> tris(n);
-    float extent = std::max(std::max(std::fabs(camera_pos[0]), std::fabs(camera_pos[1])), std::fabs(camera_pos[2]));
-    for (uint32_t i = 0; i < n; ++i) { std::memcpy(&tris[i], tri_verts + 9*size_t(i), sizeof(BuildTri)); for (int k = 0; k < 9; ++k) extent = std::max(extent, std::fabs(tri_verts[9*size_t(i) + k])); }
-    Bvh4 bvh; build_bvh4(tris.data(), n, bvh, 0, 1e-6f*extent, 4, 0.5f);
-    const std::vector<CutBox> cut = top_level_cut(bvh, 16);
-    const uint32_t need = traversal_stack_need(bvh, cut);
-    if (stack_need) *stack_need = need;
-    if (need > (stack_size ? stack_size : uint32_t(kStackSize))) return TGB_ERR_UNSUPPORTED;
-    QBvh4 qb; quantize_bvh4(bvh, qb, ~int32_t(n << 3));
-    std::vector<int32_t> new_index(qb.old_index.size()), cut_link(cut.size());
-    for (size_t i = 0; i < qb.old_index.size(); ++i) new_index[size_t(qb.old_index[i])] = int32_t(i);
-    for (size_t i = 0; i < cut.size(); ++i) cut_link[i] = cut[i].link >= 0 ? new_index[size_t(cut[i].link)] : cut[i].link;
+    SceneBvh sb;
+    build_triangle_scene_bvh(tri_verts, n, std::max(std::max(std::fabs(camera_pos[0]), std::fabs(camera_pos[1])), std::fabs(camera_pos[2])), sb);
+    if (stack_need) *stack_need = sb.stack_need;
+    if (sb.stack_need > (stack_size ? stack_size : uint32_t(kStackSize))) return TGB_ERR_UNSUPPORTED;
+    const std::vector<CutBox> &cut = sb.cut; const QBvh4 &qb = sb.qtree;
     std::vector<int32_t> stack;
     for (uint32_t r = 0; r < n_queries; ++r) {
         const float *q = queries + 8*size_t(r);
         const V3 o = f3(q), d = f3(q + 3); const float tnear = q[6], tfar = q[7];
-        const float ooeps = 1e-30f;
-        const float inv[3] = {1.0f/(std::fabs(d.x) > ooeps ? d.x : std::copysign(ooeps, d.x)), 1.0f/(std::fabs(d.y) > ooeps ? d.y : std::copysign(ooeps, d.y)),
-                              1.0f/(std::fabs(d.z) > ooeps ? d.z : std::copysign(ooeps, d.z))};
+        float inv[3]; host_inv_dir(d, inv);
         const float oo[3] = {o.x, o.y, o.z}, ood[3] = {o.x*inv[0], o.y*inv[1], o.z*inv[2]};
         uint32_t mask = 0;                                                  // mesh_cut_test<true>
         for (size_t k = 0; k < cut.size(); ++k) {
@@ -1796,7 +1712,7 @@ int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *ca
         for (int from_cut = 0; from_cut < 2; ++from_cut) {
             uint32_t *c4 = o10 + 2 + 4*from_cut;
             stack.clear();
-            if (from_cut) { for (int k = int(cut.size()) - 1; k >= 0; --k) if (mask & (1u << k)) stack.push_back(cut_link[size_t(k)]); }
+            if (from_cut) { for (int k = int(cut.size()) - 1; k >= 0; --k) if (mask & (1u << k)) stack.push_back(cut[size_t(k)].link); }
             else stack.push_back(0);
             bool occluded = false;
             int32_t cur = stack.back(); stack.pop_back();
@@ -1821,7 +1737,7 @@ int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *ca
                     for (uint32_t i = 0; i < count && !occluded; ++i) {
                         c4[3]++;
                         float best = tfar;
-                        if (first + i < n) occluded = host_triangle(tris[bvh.order[first + i]], o, d, tnear, best);
+                        occluded = host_triangle(sb.isect[first + i], o, d, tnear, best);
                     }
                     if (occluded) break;
                 }
