@@ -319,6 +319,29 @@ int  tgb200_choose_light_probe(tgb_ctx *ctx, uint32_t seed, uint32_t n, const ui
  * (0: no query, 1: settled by the analytic / cut pass, 2: reached the BVH pass), traced as a blocker test.  A failed probe
  * still restores them unless the device itself faulted.  The context's control block and ray counters are left as they were. */
 int  tgb200_shadow_probe(tgb_ctx *ctx, uint32_t n, const float *query, const int *light_mis, float *out);
+/* tgb200_bounce_probe: one iteration of the wavefront loop -- the path ray's closest hit, the shading kernel the context renders
+ * with, the shadow kernels and the fold into the path -- for n path states.  A state is a record of TGB_BOUNCE_WORDS 32-bit
+ * words (float unless marked):
+ *   [TGB_BR_ORIGIN + 0..2]  ray origin        [TGB_BR_TMIN]        ray tmin
+ *   [TGB_BR_DIR + 0..2]     ray direction     [TGB_BR_STATUS]      uint: out 1 = alive, 0 = finished (ignored on input)
+ *   [TGB_BR_THROUGHPUT+0..2] throughput       [TGB_BR_BOUNCE]      uint: bounce of the ray
+ *   [TGB_BR_EMISSION + 0..2] radiance so far  [TGB_BR_FLAGS]       uint: bit 0 = wasSpecular
+ *   [TGB_BR_PIXEL]  uint: pixel id (x + y*width)   [TGB_BR_SEED] uint: sampler seed of the pixel's tile
+ *   [TGB_BR_SAMPLE] uint: sample index             [TGB_BR_DIMENSION] uint: the sampler's next Sobol dimension
+ *   [TGB_BR_PCG + 0..1] uint: the supplemental PCG state (low word first); the remaining words are zero.
+ * An alive input is a path about to trace its ray at `bounce` (< maxBounces; other inputs are refused with TGB_ERR_INVALID).  The
+ * states enter the loop as survivors just handed over: they are binned by ray-coherence key and traced in key order, and those
+ * that miss the BVH's top-level cut keep their analytic hit, as in a render.  An alive output is the next state, as the survivor
+ * hand-off stores it.  A finished output holds the sample's radiance in EMISSION, the sampler's dimension and PCG state after
+ * the bounce, and the input's other fields.  Runs in chunks of half the context's capacity on its first wavefront; the
+ * context's control block and ray counters are left as they were. */
+enum { TGB_BR_ORIGIN = 0, TGB_BR_TMIN = 3, TGB_BR_DIR = 4, TGB_BR_STATUS = 7, TGB_BR_THROUGHPUT = 8, TGB_BR_BOUNCE = 11,
+       TGB_BR_EMISSION = 12, TGB_BR_FLAGS = 15, TGB_BR_PIXEL = 16, TGB_BR_SEED = 17, TGB_BR_SAMPLE = 18, TGB_BR_DIMENSION = 19,
+       TGB_BR_PCG = 20, TGB_BOUNCE_WORDS = 24 };
+int  tgb200_bounce_probe(tgb_ctx *ctx, uint32_t n, const uint32_t *state_in, uint32_t *state_out);
+/* tgb200_shade_variant: the shading kernel the context renders (and tgb200_bounce_probe runs) with, as its template arguments:
+ * variant[0] = curves, variant[1] = material sort, variant[2] = lobe set (1: the Lambert-only instantiation). */
+int  tgb200_shade_variant(const tgb_ctx *ctx, uint32_t *variant);
 /* tgb200_abort cancels the render in progress (it returns TGB_ERR_ABORTED) or, if none is running, the next one -- so an
  * abort that lands between an asynchronous start and the worker reaching the render call is not lost.  A caller that
  * starts renders asynchronously calls tgb200_clear_abort before spawning the worker (the adapter's startRender does).   */

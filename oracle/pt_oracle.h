@@ -55,6 +55,11 @@ int      oracle_light_probe_mode(oracle_scene *s, int prim, uint32_t seed, uint3
                                  const float *p, float *out);
 int      oracle_choose_light(oracle_scene *s, uint32_t seed, int n, const uint32_t *pixel_id, uint32_t sample, const float *p, float *out);
 int      oracle_shadow_probe(oracle_scene *s, int n, const float *query, const int *light_mis, float *out);
+/* tgb200_bounce_probe's twin on records of TGB_BOUNCE_WORDS words.  camera = 0: one iteration of traceSample's loop from each
+ * state (the sampler resumes at the record's dimension and PCG state); camera = 1: the camera state of (pixel, sample) for the
+ * record's seed, the input of bounce 0 (only PIXEL, SEED and SAMPLE are read).  Returns -1 (nothing written) when a state to
+ * step has bounce >= maxBounces. */
+int      oracle_bounce_probe(oracle_scene *s, int camera, int n, const uint32_t *in, uint32_t *out);
 int      oracle_hair_eval(float roughness, float scale_angle_deg, const float *sigma_a, const float *wi_wo, int n, float *out);
 int      oracle_hair_tables(float roughness, float scale_angle_deg, const float *sigma_a, float *tables, float *sums, float *v);
 

@@ -57,6 +57,8 @@ def lib():
         L.oracle_choose_light.argtypes = [vp, u32, C.c_int, vp, u32, vp, vp]
         L.oracle_shadow_probe.restype = C.c_int
         L.oracle_shadow_probe.argtypes = [vp, C.c_int, vp, vp, vp]
+        L.oracle_bounce_probe.restype = C.c_int
+        L.oracle_bounce_probe.argtypes = [vp, C.c_int, C.c_int, vp, vp]
         _LIB = L
     return _LIB
 
@@ -112,6 +114,16 @@ class Oracle:
         hits = (abi.Hit*len(rays))()
         lib().oracle_trace_closest(self.h, rays.ctypes.data, hits, len(rays))
         return np.ctypeslib.as_array(hits).copy() if len(rays) else np.zeros(0)
+
+    def bounce(self, states, camera=False):
+        """oracle_bounce_probe: uint32 [n, abi.BOUNCE_WORDS] path states in, the states after one loop iteration out
+        (camera=True: the camera states of the records' (pixel, seed, sample))."""
+        states = np.ascontiguousarray(states, dtype=np.uint32).reshape(-1, abi.BOUNCE_WORDS)
+        out = np.zeros_like(states)
+        rc = lib().oracle_bounce_probe(self.h, 1 if camera else 0, len(states), states.ctypes.data, out.ctypes.data)
+        if rc != 0:
+            raise RuntimeError("oracle_bounce_probe -> %d" % rc)
+        return out
 
 
 def kat_eval(which, args):

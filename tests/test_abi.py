@@ -97,6 +97,10 @@ def test_probe_hooks_refuse_a_missing_context():
     lm = np.zeros(2, np.int32)
     assert L.tgb200_shadow_probe(None, 1, buf.ctypes.data, lm.ctypes.data, buf.ctypes.data) == abi.TGB_ERR_INVALID
     assert L.tgb200_shadow_probe(None, 0, None, None, None) == abi.TGB_ERR_INVALID
+    st = np.zeros(abi.BOUNCE_WORDS, np.uint32)
+    assert L.tgb200_bounce_probe(None, 1, st.ctypes.data, st.ctypes.data) == abi.TGB_ERR_INVALID
+    assert L.tgb200_bounce_probe(None, 0, None, None) == abi.TGB_ERR_INVALID
+    assert L.tgb200_shade_variant(None, pix.ctypes.data) == abi.TGB_ERR_INVALID
 
 
 def test_product_never_imports_the_oracle():

@@ -738,23 +738,15 @@ void launch_shadow_bvh(tgb_ctx *c, const Wavefront &w, cudaStream_t st, uint32_t
     }
 }
 
-// One iteration's kernels of wavefront w on stream st.  `bound` >= the iteration's ctl.n: grids are upper bounds, the kernels
-// read the real sizes from the device-resident control block.
-void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInfo &bi, int cur, uint32_t bound, int slot, uint64_t &launches) {
-    const DScene &sc = c->sc;
-    const bool has_bvh = sc.n_nodes != 0, curves = c->has_curves;
-    PathBuf &pb = w.pb[cur], &nxt = w.pb[cur ^ 1];
-    const bool prof = c->profiling;
-    if (prof) cudaEventRecord(w.ev_k[slot][0], st);
-    k_regen<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
-    if (prof) cudaEventRecord(w.ev_k[slot][1], st);
-    if (has_bvh) {
-        uint32_t grid = std::min(blocks(bound, kTraceBlock), c->persist_blocks);
-        if (curves) k_trace<true><<<grid, kTraceBlock, 0, st>>>(sc, pb, w.order, w.ctl);
-        else k_trace<false><<<grid, kTraceBlock, 0, st>>>(sc, pb, w.order, w.ctl);
-        launches++;
-    }
-    if (prof) cudaEventRecord(w.ev_k[slot][2], st);
+// k_trace, k_shade and k_shadow_prep of wavefront w over the paths of pb, in the instantiations the context renders with (also
+// tgb200_bounce_probe's).  `bound` >= ctl.n: an upper bound of the paths.
+void launch_trace(tgb_ctx *c, const Wavefront &w, const PathBuf &pb, cudaStream_t st, uint32_t bound) {
+    const uint32_t grid = std::min(blocks(bound, kTraceBlock), c->persist_blocks);
+    if (c->has_curves) k_trace<true><<<grid, kTraceBlock, 0, st>>>(c->sc, pb, w.order, w.ctl);
+    else k_trace<false><<<grid, kTraceBlock, 0, st>>>(c->sc, pb, w.order, w.ctl);
+}
+void launch_shade(tgb_ctx *c, const Wavefront &w, const PathBuf &pb, cudaStream_t st, const BatchInfo &bi, uint32_t bound) {
+    const DScene &sc = c->sc; const bool curves = c->has_curves;
     if (c->sort_materials) {
         if (curves) k_shade<true, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
         else k_shade<false, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
@@ -763,11 +755,27 @@ void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInf
         else if (c->diffuse_only) k_shade<false, false, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
         else k_shade<false, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     }
-    launches++;
+}
+void launch_shadow_prep(tgb_ctx *c, const Wavefront &w, cudaStream_t st, uint32_t bound) {
+    if (c->has_curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(c->sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(c->sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+}
+
+// One iteration's kernels of wavefront w on stream st.  `bound` >= the iteration's ctl.n: grids are upper bounds, the kernels
+// read the real sizes from the device-resident control block.
+void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInfo &bi, int cur, uint32_t bound, int slot, uint64_t &launches) {
+    const DScene &sc = c->sc;
+    const bool has_bvh = sc.n_nodes != 0;
+    PathBuf &pb = w.pb[cur], &nxt = w.pb[cur ^ 1];
+    const bool prof = c->profiling;
+    if (prof) cudaEventRecord(w.ev_k[slot][0], st);
+    k_regen<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
+    if (prof) cudaEventRecord(w.ev_k[slot][1], st);
+    if (has_bvh) { launch_trace(c, w, pb, st, bound); launches++; }
+    if (prof) cudaEventRecord(w.ev_k[slot][2], st);
+    launch_shade(c, w, pb, st, bi, bound); launches++;
     if (prof) cudaEventRecord(w.ev_k[slot][3], st);
-    if (curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
-    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
-    launches++;
+    launch_shadow_prep(c, w, st, bound); launches++;
     if (prof) cudaEventRecord(w.ev_k[slot][4], st);
     if (has_bvh) { launch_shadow_bvh(c, w, st, std::min(blocks(2*bound, kTraceBlock), c->persist_blocks)); launches++; }
     if (prof) cudaEventRecord(w.ev_k[slot][5], st);
@@ -1916,6 +1924,80 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
     }
     if (e == cudaSuccess) e = b.download(out, dout, 8*size_t(n));
     return b.finish(e, "shadow_probe");
+}
+
+int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32_t *state_out) {
+    if (!c || (n && (!state_in || !state_out))) return TGB_ERR_INVALID;
+    const uint32_t max_bounces = c->sc.set.max_bounces;
+    for (uint32_t i = 0; i < n; ++i) {
+        const uint32_t *r = state_in + TGB_BOUNCE_WORDS*size_t(i);
+        if (r[TGB_BR_BOUNCE] >= max_bounces || r[TGB_BR_BOUNCE] > 0xFFu || r[TGB_BR_DIMENSION] > 0xFFFFu)
+            return fail(c, TGB_ERR_INVALID, "state %u: bounce %u (max_bounces %u) or dimension %u out of range", i, r[TGB_BR_BOUNCE],
+                        max_bounces, r[TGB_BR_DIMENSION]);
+    }
+    if (n == 0) return TGB_OK;
+    CU(cudaSetDevice(c->device));
+    Wavefront &w = c->wf[0];
+    if (int rc = ensure_results(c, w.capacity)) return rc;
+    ProbeBufs b(c);
+    uint32_t *din = nullptr, *dout = nullptr, *pix = nullptr; Ctl *ctl_saved = nullptr; Counters *ctr_saved = nullptr;
+    cudaError_t e = b.upload(&din, state_in, TGB_BOUNCE_WORDS*size_t(n));
+    if (e == cudaSuccess) e = b.alloc(&dout, TGB_BOUNCE_WORDS*size_t(n));
+    if (e == cudaSuccess) e = b.alloc(&pix, 4*size_t(w.capacity) + 1);
+    if (e == cudaSuccess) e = b.alloc(&ctl_saved, 1);
+    if (e == cudaSuccess) e = b.alloc(&ctr_saved, 1);
+    // the probe's paths must not show in the context's control block or in the next render's statistics
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, w.ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
+    const bool saved = e == cudaSuccess;
+    const DScene &sc = c->sc; cudaStream_t st = c->stream;
+    PathBuf &pb = w.pb[0], &dst = w.pb[1];
+    // per chunk: one pixel per path (pix_id, pix_seed, pix_first (m + 1 offsets), pix_base), so path id = result slot = its index
+    uint32_t *pix_id = pix, *pix_seed = pix + w.capacity, *pix_base = pix + 2*size_t(w.capacity), *pix_first = pix + 3*size_t(w.capacity);
+    for (uint32_t off = 0; off < n && e == cudaSuccess; off += w.capacity) {
+        const uint32_t m = std::min(w.capacity, n - off);
+        // the states enter as m survivors k_accum has just handed over, with no camera path left to issue: k_iter_end and
+        // k_bin_scatter then set up the iteration (survivor count, traversal order by ray-coherence key, culled survivors left out)
+        Ctl init; std::memset(&init, 0, sizeof(Ctl));
+        init.next_count = m; init.capacity = w.capacity;
+        e = cudaMemcpyAsync(w.ctl, &init, sizeof(Ctl), cudaMemcpyHostToDevice, st);
+        if (e == cudaSuccess) e = cudaMemsetAsync(w.bin_hist, 0, kBins*sizeof(uint32_t), st);
+        if (e != cudaSuccess) break;
+        BatchInfo bi; bi.pix_id = pix_id; bi.pix_seed = pix_seed; bi.n_pix = m; bi.spp_begin = 0;
+        bi.pix_first = pix_first; bi.pix_base = pix_base;
+        bi.pix_bits = 0; while ((1u << bi.pix_bits) < m) ++bi.pix_bits;
+        uint32_t *o = dout + TGB_BOUNCE_WORDS*size_t(off);
+        k_probe_bounce_setup<<<blocks(m, 256), 256, 0, st>>>(sc, pb, din + TGB_BOUNCE_WORDS*size_t(off), pix_id, pix_seed, pix_first,
+                                                            pix_base, w.bin_keys, w.bin_hist, o, m);
+        k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, sc.n_nodes ? 1 : 0);
+        if (sc.n_nodes) {
+            k_bin_scatter<<<blocks(m, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
+            launch_trace(c, w, pb, st, m);
+        }
+        launch_shade(c, w, pb, st, bi, m);
+        launch_shadow_prep(c, w, st, m);
+        if (sc.n_nodes) launch_shadow_bvh(c, w, st, std::min(blocks(2*m, kTraceBlock), c->persist_blocks));
+        k_accum<<<blocks(m, 256), 256, 0, st>>>(sc, pb, dst, w.sr, bi, w.ctl, w.bin_keys, w.bin_hist);
+        k_probe_bounce_alive<<<blocks(m, 256), 256, 0, st>>>(dst, w.ctl, o);
+        k_probe_bounce_finished<<<blocks(m, 256), 256, 0, st>>>(pb, c->R, o, m);
+        e = cudaGetLastError();
+        // (the next chunk's control block is copied from this host variable: wait until this one is consumed)
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    }
+    // restored also when a launch failed (the copies are queued after whatever was queued)
+    if (saved) {
+        const cudaError_t r1 = cudaMemcpyAsync(w.ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, st);
+        const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
+    }
+    if (e == cudaSuccess) e = b.download(state_out, dout, TGB_BOUNCE_WORDS*size_t(n));
+    return b.finish(e, "bounce_probe");
+}
+
+int tgb200_shade_variant(const tgb_ctx *c, uint32_t *variant) {
+    if (!c || !variant) return TGB_ERR_INVALID;
+    variant[0] = c->has_curves ? 1u : 0u; variant[1] = c->sort_materials ? 1u : 0u; variant[2] = c->diffuse_only ? 1u : 0u;
+    return TGB_OK;
 }
 
 int tgb200_clear_abort(tgb_ctx *c) {

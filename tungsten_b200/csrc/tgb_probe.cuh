@@ -1,6 +1,7 @@
 // Kernels of the test hooks (tgb200_bsdf_probe, tgb200_bsdf_sample_probe, tgb200_light_probe, tgb200_choose_light_probe,
 // tgb200_shadow_probe): one thread per input, each calling the device functions k_shade calls (bsdf_eval / bsdf_pdf / bsdf_sample
 // with k_shade's template arguments, light_sample_direct + light_hit_direct / mesh_direct_pdf, choose_light, light_query).
+// tgb200_bounce_probe's kernels only set up and read back path state around the renderer's own wavefront kernels.
 // Nothing here restates their arithmetic.
 #pragma once
 #include "tgb_wavefront.cuh"
@@ -138,6 +139,70 @@ __global__ void __launch_bounds__(128) k_probe_shadow_read(Scratch sr, const int
     const float4 x = mis ? sr.M1[i] : sr.N1[i];
     float *o = out + 8*size_t(i);
     o[2] = float(sr.vis[2*size_t(i) + (mis ? 1 : 0)]); o[3] = x.x; o[4] = x.y; o[5] = x.z;
+}
+
+// tgb200_bounce_probe, before k_iter_end: state i (TGB_BOUNCE_WORDS words, include/tgb200.h) goes into slot i of pb as k_accum hands
+// a survivor over -- the analytic part of its closest hit in T2, path id i in T3.w, its ray-coherence key (kBins: it misses the BVH's
+// top-level cut and is not traversed) in keys[i], counted in the cleared histogram -- and becomes pixel i of an adaptive BatchInfo
+// (result slot pix_first[i] = i, first sample index pix_base[i] = its sample index).  out = the input with status 0 (finished).
+__global__ void __launch_bounds__(256) k_probe_bounce_setup(DScene sc, PathBuf pb, const uint32_t *in, uint32_t *pix_id, uint32_t *pix_seed,
+                                                            uint32_t *pix_first, uint32_t *pix_base, uint32_t *keys, uint32_t *hist,
+                                                            uint32_t *out, uint32_t n) {
+    const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+    if (i == 0) pix_first[n] = n;
+    if (i >= n) return;
+    const uint32_t *r = in + TGB_BOUNCE_WORDS*size_t(i);
+    uint32_t *o = out + TGB_BOUNCE_WORDS*size_t(i);
+    for (int k = 0; k < TGB_BOUNCE_WORDS; ++k) o[k] = r[k];
+    o[TGB_BR_STATUS] = 0u;
+    const V3 org = v3(__uint_as_float(r[TGB_BR_ORIGIN]), __uint_as_float(r[TGB_BR_ORIGIN + 1]), __uint_as_float(r[TGB_BR_ORIGIN + 2]));
+    const V3 d = v3(__uint_as_float(r[TGB_BR_DIR]), __uint_as_float(r[TGB_BR_DIR + 1]), __uint_as_float(r[TGB_BR_DIR + 2]));
+    const float tmin = __uint_as_float(r[TGB_BR_TMIN]);
+    const uint32_t info = (r[TGB_BR_DIMENSION] & 0xFFFFu) | (r[TGB_BR_BOUNCE] << 16) | ((r[TGB_BR_FLAGS] & 1u) ? F_WAS_SPECULAR : 0u) | F_ALIVE;
+    const Hit h = analytic_closest(sc, org, d, tmin, INFINITY);
+    pb.T0[i] = make_float4(org.x, org.y, org.z, tmin);
+    pb.T1[i] = make_float4(d.x, d.y, d.z, __uint_as_float(info));
+    pb.T2[i] = pack_hit(h);
+    pb.T3[i] = make_float4(__uint_as_float(r[TGB_BR_THROUGHPUT]), __uint_as_float(r[TGB_BR_THROUGHPUT + 1]),
+                           __uint_as_float(r[TGB_BR_THROUGHPUT + 2]), __uint_as_float(i));
+    pb.E[i] = make_float4(__uint_as_float(r[TGB_BR_EMISSION]), __uint_as_float(r[TGB_BR_EMISSION + 1]),
+                          __uint_as_float(r[TGB_BR_EMISSION + 2]), 0.0f);
+    pb.pcg[i] = uint64_t(r[TGB_BR_PCG]) | (uint64_t(r[TGB_BR_PCG + 1]) << 32);
+    pix_id[i] = r[TGB_BR_PIXEL]; pix_seed[i] = r[TGB_BR_SEED]; pix_first[i] = i; pix_base[i] = r[TGB_BR_SAMPLE];
+    const uint32_t key = mesh_cut_hit(sc, org, d, tmin, h.t) ? ray_bin(sc, org, d) : kBins;       // as k_accum keys a survivor
+    keys[i] = key;
+    if (key != kBins) atomicAdd(hist + key, 1u);
+}
+// after k_accum: the survivors k_accum compacted into dst, put back in input order through their path id
+__global__ void __launch_bounds__(256) k_probe_bounce_alive(PathBuf dst, const Ctl *ctl, uint32_t *out) {
+    const uint32_t t = blockIdx.x*blockDim.x + threadIdx.x;
+    if (t >= ctl->next_count) return;
+    const float4 t0 = dst.T0[t], t1 = dst.T1[t], t3 = dst.T3[t], e = dst.E[t];
+    const uint32_t info = __float_as_uint(t1.w);
+    uint32_t *o = out + TGB_BOUNCE_WORDS*size_t(__float_as_uint(t3.w));
+    o[TGB_BR_ORIGIN] = __float_as_uint(t0.x); o[TGB_BR_ORIGIN + 1] = __float_as_uint(t0.y); o[TGB_BR_ORIGIN + 2] = __float_as_uint(t0.z);
+    o[TGB_BR_TMIN] = __float_as_uint(t0.w);
+    o[TGB_BR_DIR] = __float_as_uint(t1.x); o[TGB_BR_DIR + 1] = __float_as_uint(t1.y); o[TGB_BR_DIR + 2] = __float_as_uint(t1.z);
+    o[TGB_BR_STATUS] = (info & F_ALIVE) ? 1u : 0u;
+    o[TGB_BR_THROUGHPUT] = __float_as_uint(t3.x); o[TGB_BR_THROUGHPUT + 1] = __float_as_uint(t3.y); o[TGB_BR_THROUGHPUT + 2] = __float_as_uint(t3.z);
+    o[TGB_BR_BOUNCE] = (info >> 16) & 0xFFu;
+    o[TGB_BR_EMISSION] = __float_as_uint(e.x); o[TGB_BR_EMISSION + 1] = __float_as_uint(e.y); o[TGB_BR_EMISSION + 2] = __float_as_uint(e.z);
+    o[TGB_BR_FLAGS] = (info & F_WAS_SPECULAR) ? 1u : 0u;
+    o[TGB_BR_DIMENSION] = info & 0xFFFFu;
+    const uint64_t pcg = dst.pcg[t];
+    o[TGB_BR_PCG] = uint32_t(pcg); o[TGB_BR_PCG + 1] = uint32_t(pcg >> 32);
+}
+// ... and the finished ones: the radiance k_accum wrote to R, the sampler state k_shade left in the path's slot
+__global__ void __launch_bounds__(256) k_probe_bounce_finished(PathBuf pb, const float4 *R, uint32_t *out, uint32_t n) {
+    const uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t *o = out + TGB_BOUNCE_WORDS*size_t(i);
+    if (o[TGB_BR_STATUS]) return;
+    const float4 c = R[i];
+    o[TGB_BR_EMISSION] = __float_as_uint(c.x); o[TGB_BR_EMISSION + 1] = __float_as_uint(c.y); o[TGB_BR_EMISSION + 2] = __float_as_uint(c.z);
+    o[TGB_BR_DIMENSION] = __float_as_uint(pb.T1[i].w) & 0xFFFFu;
+    const uint64_t pcg = pb.pcg[i];
+    o[TGB_BR_PCG] = uint32_t(pcg); o[TGB_BR_PCG + 1] = uint32_t(pcg >> 32);
 }
 
 __global__ void __launch_bounds__(128) k_probe_choose_light(DScene sc, uint32_t seed, const uint32_t *pixel_id, uint32_t sample,

@@ -1110,6 +1110,8 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
             // forward-transparency coin flip: transparency == 0 for every lobe in scope, the draw is still made (:525-529)
             (void)sampler_boolean(smp, 0.0f);
 
+            // TODO(open deviation, tests/test_gpu_bounce.py _NAN_THR): handleSurface adds estimateDirect(...)*throughput even when
+            // the estimate is zero, which is NaN for a non-finite throughput; here a bounce without shadow queries adds nothing.
             if (set.enable_light_sampling && bounce < set.max_bounces - 1) {
                 // estimateDirect -> chooseLight -> sampleDirect (TraceBase.cpp:483-494,416-459,383-400)
                 float weight;

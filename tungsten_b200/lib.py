@@ -54,6 +54,8 @@ def load():
     L.tgb200_light_probe.argtypes = [vp, i32, u32, u32, u32, vp, vp]
     L.tgb200_choose_light_probe.argtypes = [vp, u32, u32, vp, u32, vp, vp]
     L.tgb200_shadow_probe.argtypes = [vp, u32, vp, vp, vp]
+    L.tgb200_bounce_probe.argtypes = [vp, u32, vp, vp]
+    L.tgb200_shade_variant.argtypes = [vp, vp]
     L.tgb200_destroy.argtypes = [vp]; L.tgb200_destroy.restype = None
     L.tgb200_last_error.argtypes = [vp]; L.tgb200_last_error.restype = C.c_char_p
     L.tgb200_abi_version.restype = u32
@@ -145,6 +147,19 @@ class Context:
         hits = (abi.Hit*max(len(rays), 1))()
         self._check(self.L.tgb200_trace_closest(self.h, rays.ctypes.data, hits, len(rays)))
         return np.ctypeslib.as_array(hits)[:len(rays)].copy()
+
+    def bounce_probe(self, states):
+        """tgb200_bounce_probe: uint32 [n, abi.BOUNCE_WORDS] path states in, the states after one wavefront iteration out."""
+        states = np.ascontiguousarray(states, dtype=np.uint32).reshape(-1, abi.BOUNCE_WORDS)
+        out = np.zeros_like(states)
+        self._check(self.L.tgb200_bounce_probe(self.h, len(states), states.ctypes.data, out.ctypes.data))
+        return out
+
+    def shade_variant(self):
+        """The k_shade instantiation the context renders with, as its template arguments: '<CURVES, MATSORT, LS>'."""
+        v = np.zeros(3, np.uint32)
+        self._check(self.L.tgb200_shade_variant(self.h, v.ctypes.data))
+        return "<%s, %s, %d>" % ("true" if v[0] else "false", "true" if v[1] else "false", int(v[2]))
 
     def stats(self):
         s = abi.Stats()
