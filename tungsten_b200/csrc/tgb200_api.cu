@@ -1537,6 +1537,11 @@ int tgb200_shard_tiles(const tgb_tile *tiles, uint32_t n_tiles, uint32_t *order)
 namespace {
 // UniformSampler (sampling/UniformSampler.hpp:40-52): the integrator's own PCG32 stream (tile seeds, adaptive distribution)
 inline float pcg_next1d(uint64_t &state) { return normalized_uint(pcg_next(state)); }
+// Tungsten's min / max (math/MathUtil.hpp:10-26): a < b ? a : b and a > b ? a : b.  They agree with std::min / std::max on
+// numbers but not on NaN: a block whose mean overflowed to Inf has a NaN error estimate, and min(NaN, maxError) = maxError
+// gives it the largest weight, where std::min would carry the NaN into the dilation and the sample budget.
+inline float tungsten_min(float a, float b) { return a < b ? a : b; }
+inline float tungsten_max(float a, float b) { return a > b ? a : b; }
 }
 
 // PathTraceIntegrator::generateWork (PathTraceIntegrator.cpp:44-134), host only: advances every block's sample index, then
@@ -1556,24 +1561,24 @@ int tgb200_generate_work(tgb_sample_record *records, uint32_t res_x, uint32_t re
         for (size_t i = 0; i < n; ++i) {
             tgb_sample_record &r = records[i];
             float variance = r.running_variance/float(r.sample_count - 1u);              // SampleRecord::variance (uint32 arithmetic, then float)
-            r.adaptive_weight = variance/(float(r.sample_count)*std::max(r.mean*r.mean, 1e-3f));
+            r.adaptive_weight = variance/(float(r.sample_count)*tungsten_max(r.mean*r.mean, 1e-3f));
             if (r.adaptive_weight > 0.0f) errors.push_back(r.adaptive_weight);
         }
         if (errors.empty()) return 0;
         std::sort(errors.begin(), errors.end());
         const float max_error = errors[(errors.size()*95)/100];
         if (max_error == 0.0f) return 0;
-        for (size_t i = 0; i < n; ++i) records[i].adaptive_weight = std::min(records[i].adaptive_weight, max_error);
+        for (size_t i = 0; i < n; ++i) records[i].adaptive_weight = tungsten_min(records[i].adaptive_weight, max_error);
         // dilateAdaptiveWeights (:61-88)
         for (uint32_t y = 0; y < var_h; ++y) for (uint32_t x = 0; x < var_w; ++x) {
             size_t idx = x + size_t(y)*var_w;
-            if (y < var_h - 1) records[idx].adaptive_weight = std::max(records[idx].adaptive_weight, records[idx + var_w].adaptive_weight);
-            if (x < var_w - 1) records[idx].adaptive_weight = std::max(records[idx].adaptive_weight, records[idx + 1].adaptive_weight);
+            if (y < var_h - 1) records[idx].adaptive_weight = tungsten_max(records[idx].adaptive_weight, records[idx + var_w].adaptive_weight);
+            if (x < var_w - 1) records[idx].adaptive_weight = tungsten_max(records[idx].adaptive_weight, records[idx + 1].adaptive_weight);
         }
         for (int y = int(var_h) - 1; y >= 0; --y) for (int x = int(var_w) - 1; x >= 0; --x) {
             size_t idx = size_t(x) + size_t(y)*var_w;
-            if (y > 0) records[idx].adaptive_weight = std::max(records[idx].adaptive_weight, records[idx - var_w].adaptive_weight);
-            if (x > 0) records[idx].adaptive_weight = std::max(records[idx].adaptive_weight, records[idx - 1].adaptive_weight);
+            if (y > 0) records[idx].adaptive_weight = tungsten_max(records[idx].adaptive_weight, records[idx - var_w].adaptive_weight);
+            if (x > 0) records[idx].adaptive_weight = tungsten_max(records[idx].adaptive_weight, records[idx - 1].adaptive_weight);
         }
         // distributeAdaptiveSamples (:90-112)
         double total_weight = 0.0;
