@@ -339,8 +339,10 @@ enum { TGB_BR_ORIGIN = 0, TGB_BR_TMIN = 3, TGB_BR_DIR = 4, TGB_BR_STATUS = 7, TG
        TGB_BR_EMISSION = 12, TGB_BR_FLAGS = 15, TGB_BR_PIXEL = 16, TGB_BR_SEED = 17, TGB_BR_SAMPLE = 18, TGB_BR_DIMENSION = 19,
        TGB_BR_PCG = 20, TGB_BOUNCE_WORDS = 24 };
 int  tgb200_bounce_probe(tgb_ctx *ctx, uint32_t n, const uint32_t *state_in, uint32_t *state_out);
-/* tgb200_shade_variant: the shading kernel the context renders (and tgb200_bounce_probe runs) with, as its template arguments:
- * variant[0] = curves, variant[1] = material sort, variant[2] = lobe set (1: the Lambert-only instantiation). */
+/* tgb200_shade_variant: the shading kernel the context renders (and tgb200_bounce_probe runs) with, as its template arguments,
+ * into variant[0..3]: variant[0] = curves, variant[1] = material sort, variant[2] = lobe set (1: the Lambert-only
+ * instantiation), variant[3] = emitter set (1: the Lambert-only instantiation for scenes whose lights are all quads, with no
+ * infinite emitter and only constant albedo and emission textures). */
 int  tgb200_shade_variant(const tgb_ctx *ctx, uint32_t *variant);
 /* tgb200_abort cancels the render in progress (it returns TGB_ERR_ABORTED) or, if none is running, the next one -- so an
  * abort that lands between an asynchronous start and the worker reaching the render call is not lost.  A caller that

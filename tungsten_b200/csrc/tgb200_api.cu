@@ -78,6 +78,7 @@ struct tgb_ctx {
     bool mesh_lights = false;       // a mesh is a light: closest-hit shadow queries exist, k_shadow_bvh<., false> runs
     uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels (per wavefront)
     bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
+    bool quad_emitters = false;     // ... and only quad lights, constant textures: k_shade<.., .., 1, 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
     bool has_curves = false;        // selects the kernel instantiations with the curve-segment test and per-hit epsilon
     int n_bsdfs = 0; std::vector<uint32_t> prim_types; std::vector<int> light_ids;   // host copies for the test hooks' argument checks
@@ -600,9 +601,17 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         if ((rc = dev_upload(c, &qn, sb.qtree.nodes))) return rc;
         sc.qnodes = reinterpret_cast<const uint4 *>(qn); sc.qy = 0x3F80u;
     }
-    std::vector<uint32_t> sobol(1024*32);
-    std::memcpy(sobol.data(), tgb_sobol_blob, sobol.size()*4);
-    if ((rc = dev_upload(c, &sc.sobol, sobol))) return rc;
+    {   // the direction matrices, then per dimension the XOR of the columns of every low byte (sampler_next1d): 1 MiB
+        std::vector<uint32_t> sobol(size_t(kSobolLowTable) + size_t(kSobolDims)*256);
+        std::memcpy(sobol.data(), tgb_sobol_blob, size_t(kSobolLowTable)*4);
+        for (uint32_t dim = 0; dim < kSobolDims; ++dim) {
+            const uint32_t *m = sobol.data() + dim*32u;
+            uint32_t *lo = sobol.data() + kSobolLowTable + dim*256u;
+            lo[0] = 0u;
+            for (uint32_t b = 1; b < 256; ++b) lo[b] = lo[b & (b - 1)] ^ m[__builtin_ctz(b)];
+        }
+        if ((rc = dev_upload(c, &sc.sobol, sobol))) return rc;
+    }
     sc.n_prims = uint32_t(prims.size()); sc.n_lights = int(lights.size()); sc.n_inf_lights = int(inf_lights.size());
     sc.n_analytic = analytic_in_bvh ? 0 : int(analytic.size()); sc.analytic_base = analytic_in_bvh ? int(sb.isect.size()) : 0x7fffffff;
     sc.n_nodes = uint32_t(bvh.nodes.size()); sc.n_tris = uint32_t(btris.size());
@@ -623,6 +632,24 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
         const char *ls = getenv("TGB_LOBE_SET");
         c->diffuse_only = (types & ~(1u << TGB_BSDF_LAMBERT)) == 0 && !c->has_curves && !(ls && ls[0] == '0');
         if (c->diffuse_only) c->sort_materials = false;
+        // ... and every light a quad, no infinite emitter, every BSDF albedo and emission texture constant: the emitter-set-1
+        // instantiation of it (k_shade<false, false, 1, 1>: the same arithmetic without the other emitters' and textures' code)
+        bool quads = c->diffuse_only && inf_lights.empty() && TGB_QUAD_EMITTERS;
+        for (int li : lights) quads = quads && prims[size_t(li)].type == TGB_PRIM_QUAD;
+        for (const DPrim &p : prims) quads = quads && (p.emission_tex < 0 || dtex[size_t(p.emission_tex)].type == TGB_TEX_CONSTANT);
+        for (const DBsdf &b : bsdfs) quads = quads && (b.type != TGB_BSDF_LAMBERT || dtex[size_t(b.albedo_tex)].type == TGB_TEX_CONSTANT);
+        c->quad_emitters = quads;
+        if (quads) {    // its BSDFs as 16-byte records: constant albedo, type | lobes << 16 (lambert_rec)
+            std::vector<float4> lam(bsdfs.size());
+            for (size_t i = 0; i < bsdfs.size(); ++i) {
+                const DBsdf &b = bsdfs[i];
+                const V3 a = dtex[size_t(b.albedo_tex)].value;
+                const uint32_t w = (b.type & 0xFFFFu) | (b.lobes << 16);
+                float wf; std::memcpy(&wf, &w, 4);
+                lam[i] = make_float4(a.x, a.y, a.z, wf);
+            }
+            if ((rc = dev_upload(c, &sc.lambert, lam))) return rc;
+        }
     }
     return TGB_OK;
 }
@@ -752,6 +779,7 @@ void launch_shade(tgb_ctx *c, const Wavefront &w, const PathBuf &pb, cudaStream_
         else k_shade<false, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     } else {
         if (curves) k_shade<true, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
+        else if (c->quad_emitters) k_shade<false, false, 1, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
         else if (c->diffuse_only) k_shade<false, false, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
         else k_shade<false, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     }
@@ -2002,6 +2030,7 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
 int tgb200_shade_variant(const tgb_ctx *c, uint32_t *variant) {
     if (!c || !variant) return TGB_ERR_INVALID;
     variant[0] = c->has_curves ? 1u : 0u; variant[1] = c->sort_materials ? 1u : 0u; variant[2] = c->diffuse_only ? 1u : 0u;
+    variant[3] = c->quad_emitters ? 1u : 0u;
     return TGB_OK;
 }
 

@@ -140,7 +140,8 @@ struct DScene {
     // every query at the root instead (TGB_SHADOW_CUT_ENTRY=0, for A/B comparisons)
     int32_t cut_link[16]; int cut_entry;
     V3 bin_lo, bin_inv;         // ray-binning grid over the scene bounds: cell = (o - bin_lo)*bin_inv, 16 cells per axis
-    const uint32_t *sobol;      // 1024 x 32 direction matrices
+    const uint32_t *sobol;      // 1024 x 32 direction matrices, then the 1024 x 256 low-byte table (sampler_next1d)
+    const float4 *lambert;      // k_shade's emitter set 1 only: per BSDF its constant albedo and type | lobes << 16 (lambert_rec)
 };
 
 // ---------------------------------------------------------------- sampler
@@ -156,11 +157,16 @@ TGB_D void sampler_start(Sampler &s, const uint32_t *sobol, uint32_t tile_seed, 
 }
 TGB_D float sampler_pcg1d(Sampler &s) { return normalized_uint(pcg_next(s.pcg)); }
 TGB_D bool sampler_boolean(Sampler &s, float p_true) { return sampler_pcg1d(s) < p_true; }
+// The value is scramble ^ the XOR of the matrix columns of the set bits of index' = (index & ~0xFF) | ((index + scramble) & 0xFF)
+// (thirdparty/sobol/sobol.h:39-53).  The two parts of index' share no bits and XOR is associative and commutative, so the low
+// byte's columns come from one load of a table of all 256 of their XORs (kSobolLowTable words after the matrices), and only
+// the high bits -- zero to two set bits at the usual sample counts, nearly uniform across a warp -- walk the matrix.
+constexpr uint32_t kSobolDims = 1024, kSobolLowTable = kSobolDims*32u;
 TGB_D float sampler_next1d(Sampler &s) {
-    if (s.dimension >= 1024) return sampler_pcg1d(s);
-    uint32_t index = (s.index & ~0xFFu) | ((s.index + s.scramble) & 0xFFu);
-    uint32_t result = s.scramble;
-    const uint32_t *m = s.sobol + s.dimension*32u;                                    // thirdparty/sobol/sobol.h:39-53
+    if (s.dimension >= kSobolDims) return sampler_pcg1d(s);
+    uint32_t result = s.scramble ^ __ldg(s.sobol + kSobolLowTable + s.dimension*256u + ((s.index + s.scramble) & 0xFFu));
+    uint32_t index = s.index & ~0xFFu;
+    const uint32_t *m = s.sobol + s.dimension*32u;
     s.dimension++;
     while (index) {
         int b = __ffs(int(index)) - 1;
@@ -175,8 +181,10 @@ TGB_D V3 bitmap_texel(const DTex &t, int x, int y) {
     const float *p = t.texels + 3*(size_t(y)*t.res_u + x);
     return v3(__ldg(p), __ldg(p + 1), __ldg(p + 2));
 }
+// CONST: every texture the caller can reach is constant (emitter set 1, k_shade): the lookups are compiled out
+template <bool CONST = false>
 TGB_D V3 tex_eval(const DTex &t, float u, float v) {
-    if (t.type == TGB_TEX_CONSTANT) return t.value;                                   // textures/ConstantTexture.cpp:50-58
+    if (CONST || t.type == TGB_TEX_CONSTANT) return t.value;                          // textures/ConstantTexture.cpp:50-58
     if (t.type == TGB_TEX_CHECKER) {                                                  // textures/CheckerTexture.cpp:64-69
         int ui = int(u*float(t.res_u)), vi = int(v*float(t.res_v));
         return ((ui ^ vi) & 1) ? t.value : t.value2;
@@ -965,7 +973,7 @@ TGB_D float rcoat_pdf(const DScene &sc, const DBsdf &b, const Surface &s, const 
 }
 
 // LS = lobe set the kernel is compiled for: 0 = every lobe model on the path; 1 = scenes whose surfaces are all Lambert (or the
-// null BSDF of lights): the same Lambert arithmetic without the other models' code (k_shade<.., .., 1>: no spills at 64 registers)
+// null BSDF of lights): the same Lambert arithmetic without the other models' code (k_shade<.., .., 1>)
 template <bool HAIR = false, int LS = 0>
 TGB_D bool bsdf_sample(const DScene &sc, const DBsdf &b, const Surface &s, Sampler &smp, Event &e) {
     if (LS == 1) {
@@ -1074,6 +1082,36 @@ TGB_D float bsdf_pdf(const DScene &sc, const DBsdf &b, const Surface &s, const E
     return 0.0f;
 }
 
+// LS = 1 in the emitter-set-1 k_shade (every texture constant): a BSDF is one 16-byte record (DScene::lambert) instead of the
+// DBsdf -> texture chain of loads.  Same arithmetic as the LS = 1 branches of bsdf_sample / bsdf_eval / bsdf_pdf.
+struct LambertRec { uint32_t type, lobes; V3 albedo; };
+TGB_D LambertRec lambert_rec(const DScene &sc, int bsdf) {
+    const float4 r = __ldg(sc.lambert + bsdf);
+    const uint32_t w = __float_as_uint(r.w);
+    LambertRec l; l.type = w & 0xFFFFu; l.lobes = w >> 16; l.albedo = v3(r.x, r.y, r.z);
+    return l;
+}
+TGB_D bool lambert_sample(const LambertRec &b, Sampler &smp, Event &e) {
+    if (b.type != TGB_BSDF_LAMBERT) return false;                              // NullBsdf::sample() == false
+    if (!(e.requested & LOBE_DIFFUSE_R)) return false;
+    if (e.wi.z <= 0.0f) return false;
+    float xa = sampler_next1d(smp), xb = sampler_next1d(smp);
+    e.wo = cosine_hemisphere(xa, xb);
+    e.pdf = cosine_hemisphere_pdf(e.wo);
+    e.weight = b.albedo;
+    e.sampled = LOBE_DIFFUSE_R;
+    e.weight = e.weight*sqr(1.0f);
+    return true;
+}
+TGB_D V3 lambert_eval(const LambertRec &b, const Event &e) {
+    if (b.type != TGB_BSDF_LAMBERT || !(e.requested & LOBE_DIFFUSE_R) || e.wi.z <= 0.0f || e.wo.z <= 0.0f) return v3s(0.0f)*sqr(1.0f);
+    return ((b.albedo*INV_PI_F)*e.wo.z)*sqr(1.0f);
+}
+TGB_D float lambert_pdf(const LambertRec &b, const Event &e) {
+    if (b.type != TGB_BSDF_LAMBERT || !(e.requested & LOBE_DIFFUSE_R) || e.wi.z <= 0.0f || e.wo.z <= 0.0f) return 0.0f;
+    return cosine_hemisphere_pdf(e.wo);
+}
+
 // ---------------------------------------------------------------- lights
 struct LightSample { V3 d; float dist, pdf; };
 
@@ -1106,8 +1144,10 @@ TGB_D void direction_to_uv(const DPrim &p, V3 wi, float &u, float &v, float *sin
     v = acosf(-wl.y)*INV_PI_F;
 }
 
+// ES (emitter set the caller is compiled for): 0 = every light type; 1 = every light is a quad (k_shade<.., .., 1, 1>)
+template <int ES = 0>
 TGB_D bool light_sample_direct(const DScene &sc, const DPrim &l, V3 p, Sampler &smp, LightSample &out) {
-    if (l.type == TGB_PRIM_QUAD) {                                                     // primitives/Quad.cpp:172-188
+    if (ES == 1 || l.type == TGB_PRIM_QUAD) {                                          // primitives/Quad.cpp:172-188
         if (dot(l.normal, p - l.base) <= 0.0f) return false;
         float xa = sampler_next1d(smp), xb = sampler_next1d(smp);
         V3 q = l.base + l.edge0*xa + l.edge1*xb;
@@ -1186,8 +1226,9 @@ TGB_D int infinite_light_hit(const DScene &sc, V3 d) {
     return -1;
 }
 
+template <int ES = 0>
 TGB_D float light_approx_radiance(const DScene &sc, const DPrim &l, V3 p) {
-    if (l.type == TGB_PRIM_QUAD) {                                                     // primitives/Quad.cpp:256-278
+    if (ES == 1 || l.type == TGB_PRIM_QUAD) {                                          // primitives/Quad.cpp:256-278
         if (!(l.flags & PF_EMISSIVE)) return 0.0f;
         V3 R0 = l.base - p;
         if (dot(R0, l.normal) >= 0.0f) return 0.0f;
@@ -1214,6 +1255,7 @@ TGB_D float light_approx_radiance(const DScene &sc, const DPrim &l, V3 p) {
 // The reference keeps one pdf per light in a vector.  Up to 16 lights they live in registers/local memory here; beyond that
 // (any number of lights) the approximate radiances are re-evaluated in three passes -- totals, the running-total replacement of
 // the "unknown" (negative) entries, selection -- which performs the same float operations in the same order.
+template <int ES = 0>
 TGB_D int choose_light(const DScene &sc, V3 p, Sampler &smp, float &weight) {
     const int n = sc.n_lights;
     if (n == 0) return -1;
@@ -1222,7 +1264,7 @@ TGB_D int choose_light(const DScene &sc, V3 p, Sampler &smp, float &weight) {
         float pdfs[16];
         float total = 0.0f; unsigned numNonNegative = 0;
         for (int i = 0; i < n; ++i) {
-            pdfs[i] = light_approx_radiance(sc, sc.prims[sc.lights[i]], p);
+            pdfs[i] = light_approx_radiance<ES>(sc, sc.prims[sc.lights[i]], p);
             if (pdfs[i] >= 0.0f) { total += pdfs[i]; numNonNegative++; }
         }
         if (numNonNegative == 0) { for (int i = 0; i < n; ++i) pdfs[i] = 1.0f; total = float(n); }
@@ -1242,7 +1284,7 @@ TGB_D int choose_light(const DScene &sc, V3 p, Sampler &smp, float &weight) {
     }
     float known = 0.0f; unsigned numNonNegative = 0;
     for (int i = 0; i < n; ++i) {
-        const float r = light_approx_radiance(sc, sc.prims[sc.lights[i]], p);
+        const float r = light_approx_radiance<ES>(sc, sc.prims[sc.lights[i]], p);
         if (r >= 0.0f) { known += r; numNonNegative++; }
     }
     const bool none_known = numNonNegative == 0, some_unknown = numNonNegative < unsigned(n);
@@ -1250,7 +1292,7 @@ TGB_D int choose_light(const DScene &sc, V3 p, Sampler &smp, float &weight) {
     if (none_known) total = float(n);
     else if (some_unknown) {
         for (int i = 0; i < n; ++i)
-            if (light_approx_radiance(sc, sc.prims[sc.lights[i]], p) < 0.0f) total += (total == 0.0f ? 1.0f : total)/numNonNegative;
+            if (light_approx_radiance<ES>(sc, sc.prims[sc.lights[i]], p) < 0.0f) total += (total == 0.0f ? 1.0f : total)/numNonNegative;
     }
     if (total == 0.0f) return -1;
     float t = sampler_next1d(smp)*total;
@@ -1258,7 +1300,7 @@ TGB_D int choose_light(const DScene &sc, V3 p, Sampler &smp, float &weight) {
     for (int i = 0; i < n; ++i) {
         float pdf = 1.0f;
         if (!none_known) {
-            pdf = light_approx_radiance(sc, sc.prims[sc.lights[i]], p);
+            pdf = light_approx_radiance<ES>(sc, sc.prims[sc.lights[i]], p);
             if (pdf < 0.0f) { pdf = (running == 0.0f ? 1.0f : running)/numNonNegative; running += pdf; }
         }
         if (t < pdf || i == n - 1) { weight = total/pdf; return sc.lights[i]; }

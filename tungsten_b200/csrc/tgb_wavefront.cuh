@@ -703,11 +703,12 @@ TGB_D void make_surface(const DScene &sc, const Hit &h, V3 o, V3 d, Surface &s) 
     }
 }
 
-// Primitive::evalDirect (Quad.cpp:235-238, TriangleMesh.cpp:493-496, Cube evalDirect)
+// Primitive::evalDirect (Quad.cpp:235-238, TriangleMesh.cpp:493-496, Cube evalDirect); ES: the emitter set (light_sample_direct)
+template <int ES = 0>
 TGB_D V3 eval_direct(const DScene &sc, const Surface &s) {
     const DPrim &p = sc.prims[s.prim];
     if (p.emission_tex < 0 || s.backside) return v3s(0.0f);
-    return tex_eval(sc.tex[p.emission_tex], s.u, s.v);
+    return tex_eval<ES == 1>(sc.tex[p.emission_tex], s.u, s.v);
 }
 
 // light.intersect(ray) for a quad light, resolved in the shading kernel (Quad.cpp:71-99 on the light alone,
@@ -729,14 +730,15 @@ TGB_D bool quad_light_hit(const DPrim &l, V3 p, V3 d, float tnear, float &t, flo
 // infinite sphere cap or environment light (Quad.cpp:216-222,235-238; InfiniteSphereCap.cpp:173-177; InfiniteSphere.cpp:218-229,
 // 241-244).  A quad hit closer than expected_dist/(1 + 1e-3) is a miss (the NEE query passes the sampled distance, the BSDF-sampled
 // query -1).  Returns whether the light is hit; tfar = its distance (INFINITY for the infinite lights).
+template <int ES = 0>
 TGB_D bool light_hit_direct(const DScene &sc, const DPrim &l, V3 p, V3 d, float epsilon, float expected_dist, V3 &em, float &tfar,
                             float &direct_pdf) {
     em = v3s(0.0f); tfar = INFINITY;
     bool hitL = true;
-    if (l.type == TGB_PRIM_QUAD) {
+    if (ES == 1 || l.type == TGB_PRIM_QUAD) {
         float t, l0, l1; bool back;
         hitL = quad_light_hit(l, p, d, epsilon, t, l0, l1, back) && !(t*(1.0f + 1e-3f) < expected_dist);
-        if (hitL && !back) em = tex_eval(sc.tex[l.emission_tex], l0, l1);
+        if (hitL && !back) em = tex_eval<ES == 1>(sc.tex[l.emission_tex], l0, l1);
         tfar = t;
         direct_pdf = t*t/(fabsf(dot(l.normal, d))*l.area);
     } else if (l.type == TGB_PRIM_INFINITE_SPHERE_CAP) {
@@ -764,14 +766,15 @@ TGB_D float mesh_direct_pdf(const DPrim &l, V3 p, V3 d, const Surface &ls) {
 //  * mesh lights: a closest-hit query that shadow_resolve_closest finishes: x = (f, pdfL) (NEE) or x.xyz = weight (MIS), t = the
 //    sampled distance (NEE) or the BSDF pdf (MIS).
 // The MIS query keeps x.w (NEE's pdfB shares that record).
+template <int ES = 0>
 TGB_D bool light_query(const DScene &sc, const DPrim &l, V3 p, V3 d, float epsilon, bool mis, V3 f, float pdf, float pdf_b,
                        float dist, float4 &x, float &t, bool &any) {
-    if (l.type == TGB_PRIM_MESH) {
+    if (ES == 0 && l.type == TGB_PRIM_MESH) {
         any = false; x = make_float4(f.x, f.y, f.z, mis ? x.w : pdf); t = mis ? pdf : dist;
         return true;
     }
     V3 em; float tfar, directPdf;
-    const bool hitL = light_hit_direct(sc, l, p, d, epsilon, mis ? -1.0f : dist, em, tfar, directPdf);
+    const bool hitL = light_hit_direct<ES>(sc, l, p, d, epsilon, mis ? -1.0f : dist, em, tfar, directPdf);
     if (!hitL || is_zero(em)) return false;
     V3 r;
     if (mis) { r = em*f; r = r*power_heuristic(pdf, directPdf); }
@@ -942,6 +945,19 @@ __global__ void __launch_bounds__(256) k_hook_finish(DScene sc, const tgb_ray *r
 #ifndef TGB_SHADE_MINB
 #define TGB_SHADE_MINB 8
 #endif
+// ES (emitter set): 1 = every light is a quad, there is no infinite emitter and every BSDF albedo and emission texture is
+// constant; only with LS = 1.  Light selection, sampling and hits then compile the quad case alone: no mesh-light CDF search,
+// no environment importance sampling, no cap or skydome, no infinite-light lookup on misses, no checker or bitmap lookup.
+// The arithmetic and the draws are those of ES = 0.  TGB_QUAD_EMITTERS=0 builds a library that never takes it (A/B runs).
+// Its launch bounds: TGB_SHADE_MINB_QUAD blocks of 128 per SM.  At 8 blocks (64 registers) it spills 144 B per thread and
+// at 6 (80 registers) 36 B; at 5 (88 registers) nothing, and 5 measured fastest (H100, C1: 646.6 Msamples/s against 641.7
+// at 6; 8 blocks measured 8 % slower than 6 before the emitter set had its BSDF records).
+#ifndef TGB_QUAD_EMITTERS
+#define TGB_QUAD_EMITTERS 1
+#endif
+#ifndef TGB_SHADE_MINB_QUAD
+#define TGB_SHADE_MINB_QUAD 5
+#endif
 // MATSORT ("active-ray sort by material" of the path): scenes with several lobe models make the lanes of a warp run
 // different BSDF code one after the other (C2: k_shade many times slower per path than on the Lambert-only C1).  The paths of a
 // block are therefore dealt to its threads by BSDF type (block-local counting sort in shared memory: 512 consecutive
@@ -1005,8 +1021,8 @@ TGB_D void shadow_resolve_closest(const DScene &sc, const Scratch &sr, uint32_t 
     sr.vis[2*size_t(s) + (mis ? 1 : 0)] = 1u;
 }
 
-template <bool CURVES, bool MATSORT, int LS = 0>
-__global__ void __launch_bounds__(MATSORT ? kShadeSortBlock : 128, MATSORT ? 1024/kShadeSortBlock : (LS == 1 ? 6 : TGB_SHADE_MINB))
+template <bool CURVES, bool MATSORT, int LS = 0, int ES = 0>
+__global__ void __launch_bounds__(MATSORT ? kShadeSortBlock : 128, MATSORT ? 1024/kShadeSortBlock : (LS == 1 ? (ES == 1 ? TGB_SHADE_MINB_QUAD : 6) : TGB_SHADE_MINB))
 k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squeue, Counters *ctr) {
     const uint32_t n = ctl->n;
     // MATSORT: the block owns a window of kShadeSortItems x blockDim consecutive slots, counting-sorts them by BSDF type in shared
@@ -1062,7 +1078,7 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
 
         if (h.id == HID_MISS) {
             // loop exit with didHit == false: handleInfiniteLights (TraceBase.cpp:570-578, TraceableScene.hpp:194-209)
-            if (bounce >= set.min_bounces && bounce < set.max_bounces && sc.n_inf_lights > 0) {
+            if (ES == 0 && bounce >= set.min_bounces && bounce < set.max_bounces && sc.n_inf_lights > 0) {
                 int li = infinite_light_hit(sc, d);
                 if (li >= 0) {
                     const DPrim &l = sc.prims[li];
@@ -1086,6 +1102,8 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
             }
             Surface sf; make_surface<CURVES>(sc, h, o, d, sf);
             const DBsdf &b = sc.bsdfs[sf.bsdf];
+            LambertRec lb; if (ES == 1) lb = lambert_rec(sc, sf.bsdf);
+            const uint32_t lobes = ES == 1 ? lb.lobes : b.lobes;
             const float epsilon = sf.eps;                                                    // IntersectionInfo::epsilon
             int qli = 0;
 
@@ -1101,7 +1119,7 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
                     if (!is_zero(T_)) { T_ = normalize(T_); frame.n = N; frame.t = T_; frame.b = cross(N, T_); }
                 }
                 bool hitBackside = dot(frame.n, d) > 0.0f;
-                bool isTransmissive = (b.lobes & LOBE_TRANSMISSIVE) != 0;
+                bool isTransmissive = (lobes & LOBE_TRANSMISSIVE) != 0;
                 bool flipFrame = set.enable_two_sided_shading && hitBackside && !isTransmissive;
                 if (flipFrame) { frame.n = -frame.n; frame.t = -frame.t; }
                 e.frame = frame; e.wi = to_local(frame, -d); e.wo = v3s(0.0f); e.weight = v3s(1.0f); e.pdf = 1.0f;
@@ -1115,9 +1133,9 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
             if (set.enable_light_sampling && bounce < set.max_bounces - 1) {
                 // estimateDirect -> chooseLight -> sampleDirect (TraceBase.cpp:483-494,416-459,383-400)
                 float weight;
-                int li = choose_light(sc, sf.p, smp, weight);
-                bool pureSpecular = b.lobes != 0 && (b.lobes & ~uint32_t(LOBE_SPECULAR)) == 0;
-                if (li >= 0 && !pureSpecular && b.lobes != LOBE_FORWARD) {
+                int li = choose_light<ES>(sc, sf.p, smp, weight);
+                bool pureSpecular = lobes != 0 && (lobes & ~uint32_t(LOBE_SPECULAR)) == 0;
+                if (li >= 0 && !pureSpecular && lobes != LOBE_FORWARD) {
                     const DPrim &l = sc.prims[li];
                     // lightSample (TraceBase.cpp:246-285).  For quad / environment lights the light's own hit
                     // (attenuatedEmission, :160-165) and lightF (:279-284) are resolved here and the query that is
@@ -1125,17 +1143,17 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
                     float4 n1 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), m1 = make_float4(0.0f, 0.0f, 0.0f, 0.0f); float mpb = 0.0f;
                     V3 qnd = v3s(0.0f), qmd = v3s(0.0f); float qnt = INFINITY, qmt = INFINITY;
                     LightSample ls;
-                    if (light_sample_direct(sc, l, sf.p, smp, ls)) {
+                    if (light_sample_direct<ES>(sc, l, sf.p, smp, ls)) {
                         e.wo = to_local(e.frame, ls.d);
                         bool ok = true;
                         if (set.enable_consistency_checks)                                     // isConsistent (:53-60)
                             ok = (dot(ls.d, sf.Ng) < 0.0f) == ((e.wo.z < 0.0f) != e.flipped);
                         if (ok) {
                             e.requested = LOBE_ALL_BUT_SPECULAR;
-                            V3 f = bsdf_eval<CURVES, LS>(sc, b, sf, e);
+                            V3 f = ES == 1 ? lambert_eval(lb, e) : bsdf_eval<CURVES, LS>(sc, b, sf, e);
                             if (!is_zero(f)) {
-                                float pdfB = bsdf_pdf<CURVES, LS>(sc, b, sf, e);
-                                qn = light_query(sc, l, sf.p, ls.d, epsilon, false, f, ls.pdf, pdfB, ls.dist, n1, qnt, qn_any);
+                                float pdfB = ES == 1 ? lambert_pdf(lb, e) : bsdf_pdf<CURVES, LS>(sc, b, sf, e);
+                                qn = light_query<ES>(sc, l, sf.p, ls.d, epsilon, false, f, ls.pdf, pdfB, ls.dist, n1, qnt, qn_any);
                                 m1.w = pdfB;
                                 if (qn) qnd = ls.d;
                             }
@@ -1143,13 +1161,13 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
                     }
                     // bsdfSample (TraceBase.cpp:287-321)
                     e.requested = LOBE_ALL_BUT_SPECULAR;
-                    if (bsdf_sample<CURVES, LS>(sc, b, sf, smp, e) && !is_zero(e.weight)) {
+                    if ((ES == 1 ? lambert_sample(lb, smp, e) : bsdf_sample<CURVES, LS>(sc, b, sf, smp, e)) && !is_zero(e.weight)) {
                         V3 wo = to_global(e.frame, e.wo);
                         bool ok = true;
                         if (set.enable_consistency_checks)
                             ok = (dot(wo, sf.Ng) < 0.0f) == ((e.wo.z < 0.0f) != e.flipped);
                         if (ok) {
-                            qm = light_query(sc, l, sf.p, wo, epsilon, true, e.weight, e.pdf, 0.0f, -1.0f, m1, mpb, qm_any);
+                            qm = light_query<ES>(sc, l, sf.p, wo, epsilon, true, e.weight, e.pdf, 0.0f, -1.0f, m1, mpb, qm_any);
                             if (qm) { qmd = wo; qmt = mpb; }
                         }
                     }
@@ -1172,7 +1190,7 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
             float4 d1 = make_float4(0.0f, 0.0f, 0.0f, __int_as_float(qli));
             if ((prim.flags & PF_EMISSIVE) && bounce >= set.min_bounces) {
                 if (!set.enable_light_sampling || wasSpecular || !(prim.flags & PF_SAMPLABLE)) {
-                    V3 em = eval_direct(sc, sf)*thr;
+                    V3 em = eval_direct<ES>(sc, sf)*thr;
                     d1.x = em.x; d1.y = em.y; d1.z = em.z;
                     flags |= F_HAS_SURF;
                 }
@@ -1182,7 +1200,7 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
             // continuation sample (TraceBase.cpp:545-565)
             uint32_t status = 0;
             e.requested = LOBE_ALL;
-            bool cont = bsdf_sample<CURVES, LS>(sc, b, sf, smp, e);
+            bool cont = ES == 1 ? lambert_sample(lb, smp, e) : bsdf_sample<CURVES, LS>(sc, b, sf, smp, e);
             V3 wo = v3s(0.0f);
             if (cont) {
                 wo = to_global(e.frame, e.wo);

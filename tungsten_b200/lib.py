@@ -157,9 +157,15 @@ class Context:
 
     def shade_variant(self):
         """The k_shade instantiation the context renders with, as its template arguments: '<CURVES, MATSORT, LS>'."""
-        v = np.zeros(3, np.uint32)
+        v = np.zeros(4, np.uint32)
         self._check(self.L.tgb200_shade_variant(self.h, v.ctypes.data))
         return "<%s, %s, %d>" % ("true" if v[0] else "false", "true" if v[1] else "false", int(v[2]))
+
+    def shade_emitters(self):
+        """The emitter set of that instantiation (its ES argument): 1 = quad lights only, constant textures; else 0."""
+        v = np.zeros(4, np.uint32)
+        self._check(self.L.tgb200_shade_variant(self.h, v.ctypes.data))
+        return int(v[3])
 
     def stats(self):
         s = abi.Stats()
