@@ -40,6 +40,40 @@ def test_reference_binary_with_b200_integrator(name, tmp_path):
     assert close >= (0.97 if name in ("hair", "curves_plastic", "hair_sky") else 0.985)     # curve scenes: see tests/test_gpu_parity.py::test_curves_and_hair
 
 
+FIXTURES = sorted(d for d in os.listdir(G) if os.path.isfile(os.path.join(G, d, "scene.json")))
+
+
+@pytest.mark.skipif(not os.path.exists(EXE), reason="drop-in binary not built (needs the reference's sources at build time)")
+@pytest.mark.parametrize("name", FIXTURES)
+def test_dropin_image_equals_flattener_render(name, tmp_path):
+    """The adapter hands the library the flattener's desc bit for bit (tests/test_dropin_scene.py), and the library renders
+    with the same seed and tile seeds either way, so the drop-in's PFM is the Python twin's framebuffer exactly: stepped
+    3 + 3 + 2 spp through the adapter against one render_tiles call (spp stepping changes no bits,
+    tests/test_gpu_parity.py::test_incremental_spp_matches_one_shot).  The adaptive fixture goes through the adapter's
+    generateWork + tgb200_render_adaptive, against the same steps of the Integrator twin."""
+    from tungsten_b200 import integrator, lib
+    src = os.path.join(G, name)
+    for f in os.listdir(src):
+        if f != "scene.json":
+            os.symlink(os.path.join(src, f), tmp_path/f)
+    js = json.load(open(os.path.join(src, "scene.json")))
+    js["integrator"]["type"] = "b200_path_tracer"
+    fs = scene.load_scene(os.path.join(src, "scene.json"))
+    if fs.adaptive:
+        got, _ = _run_dropin(tmp_path, js, expect="Completed %d/%d spp" % (fs.spp, fs.spp))
+        want = integrator.B200PathTraceIntegrator().render(fs)
+    else:
+        js["renderer"]["spp_step"] = 3
+        got, _ = _run_dropin(tmp_path, js, expect="Completed %d/%d spp" % (fs.spp, fs.spp))
+        ctx = lib.Context(fs)
+        want, count = ctx.render_tiles(fs.spp)
+        ctx.close()
+        assert (count == fs.spp).all()
+    d = got != want
+    print(name, "pixels that differ: %d of %d" % (int(d.any(axis=2).sum()), d.shape[0]*d.shape[1]))
+    assert np.array_equal(got, want)
+
+
 def _run_dropin(tmp_path, js, name="b200.json", expect=None):
     json.dump(js, open(tmp_path/name, "w"))
     out = subprocess.run([EXE, "-t", "2", "-d", str(tmp_path/"out"), str(tmp_path/name)], stdout=subprocess.PIPE,

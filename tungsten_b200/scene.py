@@ -361,6 +361,26 @@ COMPLEX_IOR = {
     "Cu": ((0.2004376970, 0.9240334304, 1.1022119527), (3.9129485033, 2.4528477015, 2.1421879552)),
     "W":  ((4.3707029924, 3.3002972445, 2.9982666528), (3.5006778591, 2.6048652781, 2.2731930614)),
 }
+
+
+def _conductor_eta_k(b):
+    """(eta, k) of a conductor / rough_conductor: ConductorBsdf::fromJson (ConductorBsdf.cpp:37-40), RoughConductorBsdf::fromJson
+    (RoughConductorBsdf.cpp:35-39).  The constructors' own (rounded) copper constants (ConductorBsdf.cpp:20-26,
+    RoughConductorBsdf.cpp:17-25); `value.getField("eta", _eta) &&
+    value.getField("k", _k)` stores a given eta even when k is missing, and reads k only behind an eta; the table is consulted
+    only when "material" is given, and then replaces both."""
+    eta, k = (0.200438, 0.924033, 1.10221), (3.91295, 2.45285, 2.14219)
+    if "eta" in b:
+        eta = _vec3_field(b, "eta")
+        if "k" in b:
+            k = _vec3_field(b, "k")
+    if "material" in b:
+        if b["material"] not in COMPLEX_IOR:
+            raise SceneError("conductor material '%s' not in the table" % b["material"])
+        eta, k = COMPLEX_IOR[b["material"]]
+    return eta, k
+
+
 _CURVE_MODE = {"cylinder": abi.CURVE_CYLINDER, "half_cylinder": abi.CURVE_HALF_CYLINDER, "bcsdf_cylinder": abi.CURVE_BCSDF_CYLINDER}
 _DIST = {"beckmann": abi.DIST_BECKMANN, "phong": abi.DIST_PHONG, "ggx": abi.DIST_GGX}
 _FILTER = {"dirac": abi.FILTER_DIRAC, "box": abi.FILTER_BOX, "tent": abi.FILTER_TENT,
@@ -388,8 +408,9 @@ class FlatScene:
         t = abi.Texture(type=abi.TEX_CONSTANT); t.value[:] = [float(f32(x)) for x in v3(rgb)]
         self.textures.append(t); return len(self.textures) - 1
 
-    def add_texture(self, value, base_dir="."):
-        """Scene::fetchTexture (io/Scene.cpp:127-151)."""
+    def add_texture(self, value, base_dir=".", average=False):
+        """Scene::fetchTexture (io/Scene.cpp:127-151).  average: the texel conversion is TexelConversion::REQUEST_AVERAGE
+        (roughness textures, e.g. RoughConductorBsdf.cpp:42) rather than REQUEST_RGB; only bitmaps honour it (Scene.cpp:130-133)."""
         if isinstance(value, (int, float)):
             return self.add_texture_constant(f32(value))
         if isinstance(value, list):
@@ -414,6 +435,10 @@ class FlatScene:
                 img = load_rgbe(path)
             else:
                 raise SceneError("bitmap format outside the hot path: %s" % ext)
+            if average:
+                # a scalar bitmap: each texel (r + g + b)/3 in fp32 (io/ImageIO.cpp:179, applied by loadPfm/loadHdr :335,361),
+                # looked up as Vec3f(scalar) (BitmapTexture.cpp:326-345)
+                img = np.repeat(((img[..., 0:1] + img[..., 1:2]) + img[..., 2:3])/f32(3.0), 3, axis=2)
             if value.get("gamma_correct", True) is False:
                 pass  # HDR inputs are linear either way (BitmapTexture: gamma only applies to LDR)
             return self.add_bitmap_texture(img, value.get("interpolate", True), value.get("clamp", False))
@@ -440,30 +465,15 @@ class FlatScene:
             o.type = abi.BSDF_LAMBERT
         elif ty == "rough_conductor":
             o.type = abi.BSDF_ROUGH_CONDUCTOR
-            # the constructor's own (rounded) copper constants; the table is consulted only when "material" is given
-            # (RoughConductorBsdf.cpp:17-25,32-39)
-            eta, k = (0.200438, 0.924033, 1.10221), (3.91295, 2.45285, 2.14219)
-            if "eta" in b and "k" in b:
-                eta, k = _vec3_field(b, "eta"), _vec3_field(b, "k")
-            if "material" in b:
-                if b["material"] not in COMPLEX_IOR:
-                    raise SceneError("conductor material '%s' not in the table" % b["material"])
-                eta, k = COMPLEX_IOR[b["material"]]
+            eta, k = _conductor_eta_k(b)
             o.eta[:] = [float(f32(x)) for x in eta]; o.k[:] = [float(f32(x)) for x in k]
             o.distribution = _DIST[b.get("distribution", "ggx")]
-            o.roughness_tex = self.add_texture(b.get("roughness", 0.1), base_dir)
+            o.roughness_tex = self.add_texture(b.get("roughness", 0.1), base_dir, average=True)
         elif ty == "mirror":
             o.type = abi.BSDF_MIRROR
         elif ty == "conductor":
-            # ConductorBsdf ctor (ConductorBsdf.cpp:20-26): rounded copper constants; the table is consulted only for "material"
             o.type = abi.BSDF_CONDUCTOR
-            eta, k = (0.200438, 0.924033, 1.10221), (3.91295, 2.45285, 2.14219)
-            if "eta" in b and "k" in b:
-                eta, k = _vec3_field(b, "eta"), _vec3_field(b, "k")
-            if "material" in b:
-                if b["material"] not in COMPLEX_IOR:
-                    raise SceneError("conductor material '%s' not in the table" % b["material"])
-                eta, k = COMPLEX_IOR[b["material"]]
+            eta, k = _conductor_eta_k(b)
             o.eta[:] = [float(f32(x)) for x in eta]; o.k[:] = [float(f32(x)) for x in k]
         elif ty == "dielectric":
             o.type = abi.BSDF_DIELECTRIC
@@ -474,7 +484,7 @@ class FlatScene:
             o.ior = float(f32(b.get("ior", 1.5)))
             o.distribution = _DIST[b.get("distribution", "ggx")]
             o.enable_refraction = 1 if b.get("enable_refraction", True) else 0
-            o.roughness_tex = self.add_texture(b.get("roughness", 0.1), base_dir)
+            o.roughness_tex = self.add_texture(b.get("roughness", 0.1), base_dir, average=True)
         elif ty in ("plastic", "rough_plastic"):
             o.type = abi.BSDF_PLASTIC if ty == "plastic" else abi.BSDF_ROUGH_PLASTIC
             o.ior = float(f32(b.get("ior", 1.5)))
@@ -482,12 +492,12 @@ class FlatScene:
             o.sigma_a[:] = [float(x) for x in (_vec3_field(b, "sigma_a") if "sigma_a" in b else v3(0.0))]
             if ty == "rough_plastic":
                 o.distribution = _DIST[b.get("distribution", "ggx")]
-                o.roughness_tex = self.add_texture(b.get("roughness", 0.02), base_dir)
+                o.roughness_tex = self.add_texture(b.get("roughness", 0.02), base_dir, average=True)
         elif ty in ("smooth_coat", "rough_coat"):
             o.type = abi.BSDF_SMOOTH_COAT if ty == "smooth_coat" else abi.BSDF_ROUGH_COAT
             if ty == "rough_coat":                     # RoughCoatBsdf ctor (RoughCoatBsdf.cpp:15-23): ggx, roughness 0.02
                 o.distribution = _DIST[b.get("distribution", "ggx")]
-                o.roughness_tex = self.add_texture(b.get("roughness", 0.02), base_dir)
+                o.roughness_tex = self.add_texture(b.get("roughness", 0.02), base_dir, average=True)
             o.ior = float(f32(b.get("ior", 1.3)))
             o.thickness = float(f32(b.get("thickness", 1.0)))
             o.sigma_a[:] = [float(x) for x in (_vec3_field(b, "sigma_a") if "sigma_a" in b else v3(0.0))]
