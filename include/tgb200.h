@@ -286,8 +286,9 @@ int  tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays,
 /* Host-only count of the any-hit shadow walk (no GPU): builds the tree, top-level cut and records tgb200_create builds for a
  * scene of n triangles seen from camera_pos, then walks n_queries occlusion queries (8 floats each: o, d, tnear, t_light)
  * both as a sorted walk from the root and as the unsorted walk from the top-level cut boxes the segment enters.
- * out = 10 uint32 per query: cut mask, deepest stack of the cut walk, then per walk
- * (root, cut): occluded, node visits, leaf trips, triangle tests.  *stack_need = the traversal stack bound tgb200_create checks;
+ * out = 11 uint32 per query: cut mask, deepest stack of the cut walk, then per walk
+ * (root, cut): occluded, node visits, leaf trips, triangle tests, then the deepest stack of the root walk (for a query that
+ * meets no triangle, that of k_trace's closest-hit walk of the same ray).  *stack_need = the traversal stack bound tgb200_create checks;
  * TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the traversal's own stack).                                           */
 int  tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *camera_pos, const float *queries, uint32_t n_queries,
                               uint32_t stack_size, uint32_t *stack_need, uint32_t *out);

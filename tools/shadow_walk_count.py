@@ -64,7 +64,7 @@ def c1_queries(fs, rng, n):
 def walk_counts(tris, cam, q, stack_size=0):
     L = lib.load()
     tris = np.ascontiguousarray(tris, F); q = np.ascontiguousarray(q, F); cam = np.ascontiguousarray(cam, F)
-    out = np.zeros((len(q), 10), np.uint32); need = C.c_uint32(0)
+    out = np.zeros((len(q), 11), np.uint32); need = C.c_uint32(0)
     rc = L.tgb200_shadow_walk_count(tris.ctypes.data, len(tris), cam.ctypes.data, q.ctypes.data, len(q), stack_size,
                                     C.byref(need), out.ctypes.data)
     return rc, need.value, out

@@ -1720,8 +1720,9 @@ int tgb200_qbvh_selftest(const float *tri_verts, uint32_t n, const float *rays, 
 // a scene of n triangles seen from camera_pos, and walks every query (8 floats: o, d, tnear, t_light) with the kernels' node and
 // triangle arithmetic twice: as k_shadow_bvh walked any-hit queries before (children sorted near-to-far, from the root) and as it
 // walks them now (nearest child entered, the others pushed unsorted, from the cut boxes the segment enters).  A query that enters no cut box is not walked: k_shadow_prep settles it.
-// out = 10 uint32 per query: cut mask, deepest stack of the walk from the cut, then per walk (root, cut): occluded, node visits,
-// LEAF trips, triangle tests.  *stack_need = the bound tgb200_create checks; TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the
+// out = 11 uint32 per query: cut mask, deepest stack of the walk from the cut, then per walk (root, cut): occluded, node visits,
+// LEAF trips, triangle tests; last, the deepest stack of the walk from the root.  For a query that meets no triangle the root walk
+// is the closest-hit walk of k_trace (same order, same culling: its t_max never shrinks), so that column is k_trace's stack too.  *stack_need = the bound tgb200_create checks; TGB_ERR_UNSUPPORTED when it exceeds stack_size (0: the
 // traversal's stack), before any walk.
 int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *camera_pos, const float *queries, uint32_t n_queries,
                              uint32_t stack_size, uint32_t *stack_need, uint32_t *out) {
@@ -1746,8 +1747,8 @@ int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *ca
             }
             if (tmn <= tmx) mask |= 1u << k;
         }
-        uint32_t *o10 = out + 10*size_t(r);
-        std::memset(o10, 0, 10*sizeof(uint32_t));
+        uint32_t *o10 = out + 11*size_t(r);
+        std::memset(o10, 0, 11*sizeof(uint32_t));
         o10[0] = mask;
         if (!mask) continue;
         for (int from_cut = 0; from_cut < 2; ++from_cut) {
@@ -1786,7 +1787,7 @@ int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *ca
                 cur = stack.back(); stack.pop_back();
             }
             c4[0] = occluded ? 1u : 0u;
-            if (from_cut) o10[1] = uint32_t(deepest);
+            o10[from_cut ? 1 : 10] = uint32_t(deepest);
         }
     }
     return TGB_OK;
