@@ -71,6 +71,8 @@ def expected_adaptive_step(mean, count, rec, table, w, h):
         r = rec[b]
         bx, by = (b % var_w)*4, (b//var_w)*4
         n, base = int(r["next_sample_count"]), int(r["sample_index"])
+        if n == 0:
+            continue
         for y in range(by, min(by + 4, h)):
             for x in range(bx, min(bx + 4, w)):
                 if not table.covered[y, x]:

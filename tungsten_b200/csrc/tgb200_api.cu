@@ -814,32 +814,39 @@ void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInf
     if (prof) cudaEventRecord(w.ev_k[slot][7], st);
 }
 
-// `adaptive`: per-pixel sample ranges come from c->pix_first / c->pix_base (tgb200_render_adaptive), else every pixel
-// renders samples [spp_begin, spp_begin + spp_count).
-int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, bool adaptive = false, uint32_t adaptive_total = 0) {
-    if (c->n_pix == 0 || (!adaptive && spp_count == 0) || (adaptive && adaptive_total == 0)) return TGB_OK;
+// A step's finished radiances are kept per path (16 B each) until k_resolve folds them in sample order.  A pass holds at
+// most this many paths, so that buffer stays within 8 GiB.
+constexpr uint64_t kPassPaths = 512ull << 20;
+// bits of an index into a list of n pixels: a path id is (sample within the pass << index_bits) | pixel index
+inline uint32_t index_bits(uint64_t n) { uint32_t b = 0; while (b < 32 && (uint64_t(1) << b) < n) ++b; return b; }
+
+// `run`: one run of an adaptive step (single_render_adaptive): its pixels, their result-slot offsets and first sample indices,
+// `run_total` paths in one pass.  Else every pixel of the call renders samples [spp_begin, spp_begin + spp_count).
+int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const BatchInfo *run = nullptr, uint32_t run_total = 0) {
+    const uint32_t n_pix = run ? run->n_pix : c->n_pix;
+    if (n_pix == 0 || (!run && spp_count == 0) || (run && run_total == 0)) return TGB_OK;
     CU(cudaEventRecord(c->ev0, c->stream));
     uint64_t launches = 0;
     float trace_ms = 0.0f, shadow_ms = 0.0f; uint64_t trace_launches = 0, shadow_launches = 0, traversed = 0, shadow_traversed = 0;
     double kms[7] = {0, 0, 0, 0, 0, 0, 0}; uint64_t iterations = 0;
-    // a step's finished radiances are kept per path (16 B each) until k_resolve folds them in sample order;
-    // split the sample range so that this buffer stays below 8 GB and (sample within the call, pixel) fits 32 bits
-    uint32_t pix_bits = 0; while (pix_bits < 32 && (uint64_t(1) << pix_bits) < uint64_t(c->n_pix)) ++pix_bits;
+    // split the sample range into passes of at most kPassPaths paths whose (sample within the pass, pixel) fits 32 bits
+    const uint32_t pix_bits = index_bits(n_pix);
     const uint64_t max_k = uint64_t(1) << (32 - pix_bits);
-    const uint64_t max_paths = 512ull << 20;
-    uint32_t spp_sub = adaptive ? 1u : uint32_t(std::max<uint64_t>(1, std::min<uint64_t>(std::min<uint64_t>(spp_count, max_k), max_paths/c->n_pix)));
-    if (uint64_t(c->n_pix)*spp_sub > 0xFFFFFFFFull) return fail(c, TGB_ERR_UNSUPPORTED, "tile list too large");
-    if (adaptive) spp_count = 1;                               // one pass over the per-pixel ranges
+    uint32_t spp_sub = run ? 1u : uint32_t(std::max<uint64_t>(1, std::min<uint64_t>(std::min<uint64_t>(spp_count, max_k), kPassPaths/n_pix)));
+    if (uint64_t(n_pix)*spp_sub > 0xFFFFFFFFull) return fail(c, TGB_ERR_UNSUPPORTED, "tile list too large");
+    if (run) spp_count = 1;                                    // one pass over the per-pixel ranges
     const bool trace_bounces = getenv("TGB_TRACE_BOUNCES") != nullptr;
     uint64_t samples_done = 0;
     for (uint32_t s0 = 0; s0 < spp_count; s0 += spp_sub) {
         uint32_t ns = std::min(spp_sub, spp_count - s0);
-        uint32_t total = adaptive ? adaptive_total : c->n_pix*ns;
+        uint32_t total = run ? run_total : n_pix*ns;
         samples_done += total;
         int rc = ensure_results(c, total);
         if (rc) return rc;
-        BatchInfo bi; bi.pix_id = c->pix_id; bi.pix_seed = c->pix_seed; bi.n_pix = c->n_pix; bi.spp_begin = spp_begin + s0;
-        bi.pix_first = adaptive ? c->pix_first : nullptr; bi.pix_base = adaptive ? c->pix_base : nullptr; bi.pix_bits = pix_bits;
+        BatchInfo bi;
+        if (run) bi = *run;
+        else { bi.pix_id = c->pix_id; bi.pix_seed = c->pix_seed; bi.n_pix = n_pix; bi.pix_first = nullptr; bi.pix_base = nullptr; bi.pix_bits = pix_bits; }
+        bi.spp_begin = spp_begin + s0;
         // fork: wavefront 1 starts behind what the caller's stream holds so far (the previous sub-step's k_resolve reads R)
         const cudaStream_t st[2] = {c->stream, c->stream1};
         CU(cudaEventRecord(c->ev_fork, st[0]));
@@ -897,7 +904,7 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, bool adapt
         // join: k_resolve, and whatever the caller queues on its stream after this call, wait for wavefront 1
         CU(cudaEventRecord(c->ev_join, st[1]));
         CU(cudaStreamWaitEvent(st[0], c->ev_join, 0));
-        k_resolve<<<blocks(c->n_pix, 256), 256, 0, st[0]>>>(c->R, bi, ns, c->fb, c->fb_count); launches++;
+        k_resolve<<<blocks(n_pix, 256), 256, 0, st[0]>>>(c->R, bi, ns, c->fb, c->fb_count); launches++;
     }
     CU(cudaEventRecord(c->ev1, c->stream));
     CU(cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(Counters), cudaMemcpyDeviceToHost, c->stream));
@@ -1511,25 +1518,49 @@ int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
     if (rc) return rc;
     const uint32_t var_w = (c->res_x + 3)/4, var_h = (c->res_y + 3)/4, n_blocks = var_w*var_h;
     if (c->n_pix == 0) return TGB_OK;
-    if (c->adaptive_capacity < c->n_pix + 1 || !c->rec_dev) {
-        if ((rc = dev_alloc(c, &c->pix_first, size_t(c->n_pix) + 1))) return rc;
-        if ((rc = dev_alloc(c, &c->pix_base, size_t(c->n_pix) + 1))) return rc;
-        if (!c->pix_slot && (rc = dev_alloc(c, &c->pix_slot, size_t(c->res_x)*c->res_y))) return rc;
-        if (!c->rec_dev && (rc = dev_alloc(c, &c->rec_dev, n_blocks))) return rc;
-        c->adaptive_capacity = c->n_pix + 1;
-    }
-    std::vector<uint32_t> first(size_t(c->n_pix) + 1), base(size_t(c->n_pix) + 1, 0);
-    uint64_t total = 0; uint32_t max_cnt = 0;
+    std::vector<uint32_t> cnt(c->n_pix), base(size_t(c->n_pix) + 1, 0);
     for (uint32_t i = 0; i < c->n_pix; ++i) {
         const uint32_t px = c->h_pix_id[i] % c->res_x, py = c->h_pix_id[i]/c->res_x;
         const tgb_sample_record &r = records[px/4 + (py/4)*var_w];
-        first[i] = uint32_t(total); base[i] = r.sample_index;
-        total += r.next_sample_count; max_cnt = std::max(max_cnt, r.next_sample_count);
-        if (total > 0xFFFFFFFFull) return fail(c, TGB_ERR_UNSUPPORTED, "adaptive step too large");
+        cnt[i] = r.next_sample_count; base[i] = r.sample_index;
     }
-    first[c->n_pix] = uint32_t(total);
-    uint32_t pix_bits = 0; while (pix_bits < 32 && (uint64_t(1) << pix_bits) < uint64_t(c->n_pix)) ++pix_bits;
-    if (uint64_t(max_cnt) > (uint64_t(1) << (32 - pix_bits))) return fail(c, TGB_ERR_UNSUPPORTED, "adaptive step: %u samples for one pixel do not fit the path id", max_cnt);
+    // The step renders in runs of consecutive tiles of the list (the list is tile-major: a run is a range of c->pix_id), one
+    // pass each: at most kPassPaths paths, and every pixel's count fits the run's path ids.  A 4x4 block lies inside one
+    // tile, so its samples fold in one run, in renderTile's order, and the image and records do not depend on the runs.
+    struct Run { uint32_t p0, n, max_cnt; uint64_t total; };
+    const auto one_pass = [](uint32_t n, uint64_t total, uint32_t max_cnt) {
+        return total <= kPassPaths && uint64_t(max_cnt) <= (uint64_t(1) << (32 - index_bits(n)));
+    };
+    std::vector<Run> runs;
+    uint64_t step_total = 0;
+    for (uint32_t t = 0, p = 0; t < c->tiles_cached.size(); ++t) {
+        const tgb_tile &tl = c->tiles_cached[t];
+        const uint32_t n = tl.w*tl.h;
+        if (n == 0) continue;
+        uint64_t total = 0; uint32_t max_cnt = 0;
+        for (uint32_t i = p; i < p + n; ++i) { total += cnt[i]; max_cnt = std::max(max_cnt, cnt[i]); }
+        if (!one_pass(n, total, max_cnt))
+            return fail(c, TGB_ERR_UNSUPPORTED, "adaptive step: tile %u at (%u, %u) renders %llu paths, %u for one pixel: more than one pass holds",
+                        t, tl.x, tl.y, (unsigned long long)total, max_cnt);
+        if (runs.empty() || !one_pass(runs.back().n + n, runs.back().total + total, std::max(runs.back().max_cnt, max_cnt))) runs.push_back(Run{p, 0, 0, 0});
+        Run &r = runs.back();
+        r.n += n; r.total += total; r.max_cnt = std::max(r.max_cnt, max_cnt);
+        p += n; step_total += total;
+    }
+    // run k's result-slot offsets (n + 1 of them, from 0) start at pix_first[p0 + k]
+    std::vector<uint32_t> first(size_t(c->n_pix) + runs.size());
+    for (size_t k = 0; k < runs.size(); ++k) {
+        uint32_t *f = first.data() + runs[k].p0 + k, slot = 0;
+        for (uint32_t i = 0; i < runs[k].n; ++i) { f[i] = slot; slot += cnt[runs[k].p0 + i]; }
+        f[runs[k].n] = slot;
+    }
+    if (c->adaptive_capacity < first.size() || !c->rec_dev) {
+        if ((rc = dev_alloc(c, &c->pix_first, first.size()))) return rc;
+        if ((rc = dev_alloc(c, &c->pix_base, first.size()))) return rc;
+        if (!c->pix_slot && (rc = dev_alloc(c, &c->pix_slot, size_t(c->res_x)*c->res_y))) return rc;
+        if (!c->rec_dev && (rc = dev_alloc(c, &c->rec_dev, n_blocks))) return rc;
+        c->adaptive_capacity = uint32_t(first.size());
+    }
     if (!c->pix_slot_valid) {
         std::vector<uint32_t> slot(size_t(c->res_x)*c->res_y, 0xFFFFFFFFu);
         for (uint32_t i = 0; i < c->n_pix; ++i) slot[c->h_pix_id[i]] = i;
@@ -1541,12 +1572,16 @@ int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
     CU(cudaMemcpyAsync(c->pix_base, base.data(), base.size()*4, cudaMemcpyHostToDevice, c->stream));
     CU(cudaMemcpyAsync(c->rec_dev, records, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyHostToDevice, c->stream));
     CU(cudaStreamSynchronize(c->stream));                       // (the host vectors go out of scope)
-    if (total == 0) return TGB_OK;
-    if ((rc = render_device(c, 0, 0, true, uint32_t(total)))) return rc;
-    BatchInfo bi; bi.pix_id = c->pix_id; bi.pix_seed = c->pix_seed; bi.n_pix = c->n_pix; bi.spp_begin = 0;
-    bi.pix_first = c->pix_first; bi.pix_base = c->pix_base; bi.pix_bits = pix_bits;
-    k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R, bi, c->pix_slot, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
-    c->stats.kernel_launches++;
+    if (step_total == 0) return TGB_OK;
+    for (size_t k = 0; k < runs.size(); ++k) {
+        const Run &r = runs[k];
+        if (r.total == 0) continue;
+        BatchInfo bi; bi.pix_id = c->pix_id + r.p0; bi.pix_seed = c->pix_seed + r.p0; bi.n_pix = r.n; bi.spp_begin = 0;
+        bi.pix_first = c->pix_first + r.p0 + k; bi.pix_base = c->pix_base + r.p0; bi.pix_bits = index_bits(r.n);
+        if ((rc = render_device(c, 0, 0, &bi, uint32_t(r.total)))) return rc;
+        k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R, bi, c->pix_slot, r.p0, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
+        c->stats.kernel_launches++;
+    }
     CU(cudaMemcpyAsync(records, c->rec_dev, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     CU(cudaGetLastError());

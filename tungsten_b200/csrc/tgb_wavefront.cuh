@@ -804,8 +804,9 @@ TGB_D uint32_t ray_bin(const DScene &sc, V3 o, V3 d) {
 // ---- kernels ---------------------------------------------------------------------------------
 // One render call = a list of pixels (tile-major) x a sample range per pixel.  Uniform steps give every pixel the samples
 // [spp_begin, spp_begin + ns); adaptive steps (PathTraceIntegrator::generateWork, PathTraceIntegrator.cpp:110-134) give the
-// pixels of each 4x4 block their own count and first sample index.  A path carries (k << pix_bits) | pixel_list_index, k = its
-// sample's position within the call; its result slot is k*n_pix + pix (uniform) or pix_first[pix] + k (adaptive).
+// pixels of each 4x4 block their own count and first sample index.  The host renders a call in passes (sample ranges, or runs
+// of tiles for adaptive steps), and a BatchInfo describes one pass.  A path carries (k << pix_bits) | pixel_list_index, k = its
+// sample's position within the pass; its result slot is k*n_pix + pix (uniform) or pix_first[pix] + k (adaptive).
 struct BatchInfo {
     const uint32_t *pix_id, *pix_seed; uint32_t n_pix, spp_begin;
     const uint32_t *pix_first, *pix_base;       // adaptive only (else nullptr): n_pix + 1 result-slot offsets, first sample index per pixel
@@ -1492,18 +1493,19 @@ __global__ void __launch_bounds__(256) k_resolve(const float4 *R, BatchInfo bi, 
 
 // SampleRecord::addSample for every sample of an adaptive step (integrators/path_tracer/SampleRecord.hpp:44-55): one thread per
 // 4x4 variance block folds the luminance of its pixels' samples in the order renderTile produces them
-// (PathTraceIntegrator.cpp:136-156: rows, then columns, then sample index; a block never straddles a 16x16 tile).
+// (PathTraceIntegrator.cpp:136-156: rows, then columns, then sample index; a block never straddles a 16x16 tile).  bi is one
+// run of the call's pixel list, from list index pix_lo on (pix_slot holds indices into the whole list).
 struct SampleRecordD { uint32_t sample_count, next_sample_count, sample_index; float adaptive_weight, mean, running_variance; };
-__global__ void __launch_bounds__(128) k_block_stats(const float4 *R, BatchInfo bi, const uint32_t *pix_slot, uint32_t res_x, uint32_t res_y,
-                                                     uint32_t var_w, uint32_t n_blocks, SampleRecordD *rec) {
+__global__ void __launch_bounds__(128) k_block_stats(const float4 *R, BatchInfo bi, const uint32_t *pix_slot, uint32_t pix_lo, uint32_t res_x,
+                                                     uint32_t res_y, uint32_t var_w, uint32_t n_blocks, SampleRecordD *rec) {
     uint32_t b = blockIdx.x*blockDim.x + threadIdx.x;
     if (b >= n_blocks) return;
     SampleRecordD r = rec[b];
     const uint32_t bx = (b % var_w)*4u, by = (b/var_w)*4u;
     for (uint32_t y = by; y < min(by + 4u, res_y); ++y)
         for (uint32_t x = bx; x < min(bx + 4u, res_x); ++x) {
-            const uint32_t pix = pix_slot[x + y*res_x];
-            if (pix == 0xFFFFFFFFu) continue;                       // pixel not in this call's tile list
+            const uint32_t pix = pix_slot[x + y*res_x] - pix_lo;
+            if (pix >= bi.n_pix) continue;                          // pixel not in this run (0xFFFFFFFF: not in the call's tile list)
             const uint32_t first = bi.pix_first[pix], cnt = bi.pix_first[pix + 1] - first;
             for (uint32_t k = 0; k < cnt; ++k) {
                 const float4 c = R[size_t(first) + k];
