@@ -27,7 +27,7 @@ using namespace tgb;
 struct tgb_ctx;
 struct Group {
     std::vector<tgb_ctx *> members;                     // members[0] = root
-    std::vector<tgb_tile> deal_key; uint32_t deal_seed = 0;      // tile list the cached deal belongs to
+    std::vector<tgb_tile> deal_key;                      // tile list the cached deal belongs to
     std::vector<std::vector<tgb_tile>> shares;           // per member
     std::vector<uint32_t *> root_pix;                    // per member k >= 1: its share's pixel ids on the ROOT device
     std::vector<uint32_t> share_pixels;
@@ -40,10 +40,6 @@ struct Group {
 namespace {
 
 thread_local std::string g_create_error;
-
-struct DeviceBuf {
-    void *p = nullptr; size_t bytes = 0;
-};
 
 // One wavefront: the loop state of its share of a (sub)step's camera paths.  A context runs two of them, each on its own stream,
 // so that one wavefront's traversal kernels (ALU bound) run alongside the other's streaming kernels (HBM bound).
@@ -58,6 +54,16 @@ struct Wavefront {
     Ctl *h_ctl = nullptr;           // pinned: [0..3] snapshot ring (read one iteration late), [4] initial value
     cudaEvent_t ev_ring[4]{};
     cudaEvent_t ev_k[4][8]{};       // profiling: boundaries between the kernels of an iteration (regen|trace|shade|prep|shadow|accum|sort)
+};
+
+// The instantiations of the scene-dependent kernels a context runs (select_kernels), for renders and test hooks alike
+struct Kernels {
+    decltype(&k_trace<false>) trace = nullptr;
+    decltype(&k_shade<false, false>) shade = nullptr;
+    unsigned shade_block = 0, shade_paths = 0;      // k_shade's block size and paths per block
+    decltype(&k_shadow_prep<false>) shadow_prep = nullptr;
+    decltype(&k_shadow_bvh<false, false>) shadow_bvh = nullptr;
+    decltype(&k_hook_persist<false>) hook_persist = nullptr;
 };
 
 }  // namespace
@@ -81,6 +87,7 @@ struct tgb_ctx {
     bool quad_emitters = false;     // ... and only quad lights, constant textures: k_shade<.., .., 1, 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
     bool has_curves = false;        // selects the kernel instantiations with the curve-segment test and per-hit epsilon
+    Kernels ks;                     // the instantiations the five flags above select
     int n_bsdfs = 0; std::vector<uint32_t> prim_types; std::vector<int> light_ids;   // host copies for the test hooks' argument checks
     float4 *R = nullptr; size_t res_capacity = 0;   // finished radiance per path of the (sub)step
     cudaStream_t own_stream = nullptr;
@@ -654,6 +661,26 @@ int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
     return TGB_OK;
 }
 
+// The kernel instantiations of upload_scene's flags.  k_shade: material-sorted, then with curves, then the emitter set, then
+// Lambert-only, then the generic one.
+Kernels select_kernels(const tgb_ctx *c) {
+    const bool cv = c->has_curves;
+    Kernels k;
+    k.trace = cv ? k_trace<true> : k_trace<false>;
+    if (c->sort_materials) {
+        k.shade = cv ? k_shade<true, true> : k_shade<false, true>;
+        k.shade_block = kShadeSortBlock; k.shade_paths = kShadeSortBlock*kShadeSortItems;
+    } else {
+        k.shade = cv ? k_shade<true, false> : c->quad_emitters ? k_shade<false, false, 1, 1> : c->diffuse_only ? k_shade<false, false, 1> : k_shade<false, false>;
+        k.shade_block = 128; k.shade_paths = 128;
+    }
+    k.shadow_prep = cv ? k_shadow_prep<true> : k_shadow_prep<false>;
+    k.shadow_bvh = cv ? (c->mesh_lights ? k_shadow_bvh<true, true> : k_shadow_bvh<true, false>)
+                      : (c->mesh_lights ? k_shadow_bvh<false, true> : k_shadow_bvh<false, false>);
+    k.hook_persist = cv ? k_hook_persist<true> : k_hook_persist<false>;
+    return k;
+}
+
 int alloc_wavefront(tgb_ctx *c, uint32_t capacity) {
     c->capacity = capacity;
     int rc;
@@ -693,33 +720,49 @@ int alloc_wavefront(tgb_ctx *c, uint32_t capacity) {
     return TGB_OK;
 }
 
-// PathTraceIntegrator::diceTiles + the sampler seeding of prepareForRender (PathTraceIntegrator.cpp:27-42,187)
-void dice_tiles(uint32_t w, uint32_t h, uint32_t seed, std::vector<tgb_tile> &out) {
-    const uint32_t TileSize = 16;
+// The tile list of a render call: the caller's or, when n_tiles == 0, the reference's (PathTraceIntegrator::diceTiles + the
+// sampler seeding of prepareForRender, PathTraceIntegrator.cpp:27-42,187)
+std::vector<tgb_tile> call_tiles(const tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed) {
+    if (n_tiles) return std::vector<tgb_tile>(tiles, tiles + n_tiles);
+    const uint32_t TileSize = 16, w = c->res_x, h = c->res_y;
     uint64_t st = uint64_t(hash32(seed));
-    out.clear();
+    std::vector<tgb_tile> out;
     for (uint32_t y = 0; y < h; y += TileSize)
         for (uint32_t x = 0; x < w; x += TileSize) {
             tgb_tile t; t.x = x; t.y = y; t.w = std::min(TileSize, w - x); t.h = std::min(TileSize, h - y);
             t.sampler_seed = hash32(pcg_next(st));
             out.push_back(t);
         }
+    return out;
+}
+
+// a tile list equal to the one whose pixel list is already built
+bool same_tiles(const std::vector<tgb_tile> &a, const std::vector<tgb_tile> &b) {
+    return !a.empty() && a.size() == b.size() && std::memcmp(a.data(), b.data(), a.size()*sizeof(tgb_tile)) == 0;
+}
+
+// The pixel ids of a tile list, tile-major, and (pseed) each pixel's tile seed.  The tiles must lie inside the image and be
+// disjoint: k_resolve, k_unpack_tiles and k_unpack_share own one pixel per thread, and a multi-GPU context would render a pixel
+// of two tiles on two GPUs.
+int tile_pixels(tgb_ctx *c, const std::vector<tgb_tile> &tiles, std::vector<uint32_t> &pid, std::vector<uint32_t> *pseed = nullptr) {
+    pid.clear();
+    if (pseed) pseed->clear();
+    for (size_t t = 0; t < tiles.size(); ++t) {
+        const tgb_tile &tl = tiles[t];
+        if (tl.x >= c->res_x || tl.w > c->res_x - tl.x || tl.y >= c->res_y || tl.h > c->res_y - tl.y) return fail(c, TGB_ERR_INVALID, "tile %zu lies outside the image", t);
+        for (uint32_t y = 0; y < tl.h; ++y) for (uint32_t x = 0; x < tl.w; ++x) pid.push_back((tl.x + x) + (tl.y + y)*c->res_x);
+        if (pseed) pseed->resize(pid.size(), tl.sampler_seed);
+    }
+    std::vector<bool> seen(size_t(c->res_x)*c->res_y, false);
+    for (uint32_t q : pid) { if (seen[q]) return fail(c, TGB_ERR_INVALID, "tile list covers pixel %u twice", q); seen[q] = true; }
+    return TGB_OK;
 }
 
 int set_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed) {
-    std::vector<tgb_tile> own;
-    if (n_tiles == 0) { dice_tiles(c->res_x, c->res_y, seed, own); tiles = own.data(); n_tiles = uint32_t(own.size()); }
-    if (c->tiles_cached.size() == n_tiles && n_tiles && std::memcmp(c->tiles_cached.data(), tiles, n_tiles*sizeof(tgb_tile)) == 0) return TGB_OK;
+    std::vector<tgb_tile> list = call_tiles(c, tiles, n_tiles, seed);
+    if (same_tiles(list, c->tiles_cached)) return TGB_OK;
     std::vector<uint32_t> pid, pseed;
-    for (uint32_t t = 0; t < n_tiles; ++t) {
-        const tgb_tile &tl = tiles[t];
-        if (tl.x >= c->res_x || tl.w > c->res_x - tl.x || tl.y >= c->res_y || tl.h > c->res_y - tl.y) return fail(c, TGB_ERR_INVALID, "tile %u lies outside the image", t);
-        for (uint32_t y = 0; y < tl.h; ++y) for (uint32_t x = 0; x < tl.w; ++x) { pid.push_back((tl.x + x) + (tl.y + y)*c->res_x); pseed.push_back(tl.sampler_seed); }
-    }
-    {   // tiles must be disjoint: k_resolve owns one pixel per thread
-        std::vector<bool> seen(size_t(c->res_x)*c->res_y, false);
-        for (uint32_t q : pid) { if (seen[q]) return fail(c, TGB_ERR_INVALID, "tile list covers pixel %u twice", q); seen[q] = true; }
-    }
+    if (int rc = tile_pixels(c, list, pid, &pseed)) return rc;
     if (pid.size() > c->pix_capacity) {
         int rc;
         if ((rc = dev_alloc(c, &c->pix_id, pid.size()))) return rc;
@@ -733,7 +776,7 @@ int set_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed
         CU(cudaMemcpyAsync(c->pix_seed, pseed.data(), pseed.size()*4, cudaMemcpyHostToDevice, c->stream));
         CU(cudaStreamSynchronize(c->stream));
     }
-    c->tiles_cached.assign(tiles, tiles + n_tiles);
+    c->tiles_cached = std::move(list);
     return TGB_OK;
 }
 
@@ -753,44 +796,29 @@ int ensure_results(tgb_ctx *c, size_t n_paths) {
     return TGB_OK;
 }
 
-// k_shadow_bvh over the any-hit queue and (scenes with mesh lights) the closest-hit queue
-void launch_shadow_bvh(tgb_ctx *c, const Wavefront &w, cudaStream_t st, uint32_t grid) {
-    const DScene &sc = c->sc;
-    if (c->has_curves) {
-        if (c->mesh_lights) k_shadow_bvh<true, true><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
-        else k_shadow_bvh<true, false><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
-    } else {
-        if (c->mesh_lights) k_shadow_bvh<false, true><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
-        else k_shadow_bvh<false, false><<<grid, kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
-    }
+// One bounce of wavefront w's paths in pb on stream st: k_trace -> k_shade -> k_shadow_prep -> k_shadow_bvh -> k_accum (survivors
+// into nxt), as a render and tgb200_bounce_probe run it.  `bound` >= ctl.n: grids are upper bounds, the kernels read the real
+// sizes from the device-resident control block.  ev (profiling): events recorded after each of the five kernels.  Returns the
+// number of kernels launched.
+uint32_t enqueue_bounce(tgb_ctx *c, Wavefront &w, const PathBuf &pb, const PathBuf &nxt, cudaStream_t st, const BatchInfo &bi,
+                        uint32_t bound, const cudaEvent_t *ev) {
+    const DScene &sc = c->sc; const Kernels &ks = c->ks;
+    const bool has_bvh = sc.n_nodes != 0;
+    if (has_bvh) ks.trace<<<std::min(blocks(bound, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, pb, w.order, w.ctl);
+    if (ev) cudaEventRecord(ev[0], st);
+    ks.shade<<<blocks(bound, ks.shade_paths), ks.shade_block, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
+    if (ev) cudaEventRecord(ev[1], st);
+    ks.shadow_prep<<<blocks(2*bound, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+    if (ev) cudaEventRecord(ev[2], st);
+    // the any-hit queue and (scenes with mesh lights) the closest-hit queue
+    if (has_bvh) ks.shadow_bvh<<<std::min(blocks(2*bound, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
+    if (ev) cudaEventRecord(ev[3], st);
+    k_accum<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, nxt, w.sr, bi, w.ctl, w.bin_keys, w.bin_hist);
+    if (ev) cudaEventRecord(ev[4], st);
+    return has_bvh ? 5 : 3;
 }
 
-// k_trace, k_shade and k_shadow_prep of wavefront w over the paths of pb, in the instantiations the context renders with (also
-// tgb200_bounce_probe's).  `bound` >= ctl.n: an upper bound of the paths.
-void launch_trace(tgb_ctx *c, const Wavefront &w, const PathBuf &pb, cudaStream_t st, uint32_t bound) {
-    const uint32_t grid = std::min(blocks(bound, kTraceBlock), c->persist_blocks);
-    if (c->has_curves) k_trace<true><<<grid, kTraceBlock, 0, st>>>(c->sc, pb, w.order, w.ctl);
-    else k_trace<false><<<grid, kTraceBlock, 0, st>>>(c->sc, pb, w.order, w.ctl);
-}
-void launch_shade(tgb_ctx *c, const Wavefront &w, const PathBuf &pb, cudaStream_t st, const BatchInfo &bi, uint32_t bound) {
-    const DScene &sc = c->sc; const bool curves = c->has_curves;
-    if (c->sort_materials) {
-        if (curves) k_shade<true, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
-        else k_shade<false, true><<<blocks(bound, kShadeSortBlock*kShadeSortItems), kShadeSortBlock, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
-    } else {
-        if (curves) k_shade<true, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
-        else if (c->quad_emitters) k_shade<false, false, 1, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
-        else if (c->diffuse_only) k_shade<false, false, 1><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
-        else k_shade<false, false><<<blocks(bound, 128), 128, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
-    }
-}
-void launch_shadow_prep(tgb_ctx *c, const Wavefront &w, cudaStream_t st, uint32_t bound) {
-    if (c->has_curves) k_shadow_prep<true><<<blocks(2*bound, 256), 256, 0, st>>>(c->sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
-    else k_shadow_prep<false><<<blocks(2*bound, 256), 256, 0, st>>>(c->sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
-}
-
-// One iteration's kernels of wavefront w on stream st.  `bound` >= the iteration's ctl.n: grids are upper bounds, the kernels
-// read the real sizes from the device-resident control block.
+// One iteration's kernels of wavefront w on stream st: k_regen, a bounce, and the ray-coherence binning of the survivors
 void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInfo &bi, int cur, uint32_t bound, int slot, uint64_t &launches) {
     const DScene &sc = c->sc;
     const bool has_bvh = sc.n_nodes != 0;
@@ -799,16 +827,7 @@ void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInf
     if (prof) cudaEventRecord(w.ev_k[slot][0], st);
     k_regen<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
     if (prof) cudaEventRecord(w.ev_k[slot][1], st);
-    if (has_bvh) { launch_trace(c, w, pb, st, bound); launches++; }
-    if (prof) cudaEventRecord(w.ev_k[slot][2], st);
-    launch_shade(c, w, pb, st, bi, bound); launches++;
-    if (prof) cudaEventRecord(w.ev_k[slot][3], st);
-    launch_shadow_prep(c, w, st, bound); launches++;
-    if (prof) cudaEventRecord(w.ev_k[slot][4], st);
-    if (has_bvh) { launch_shadow_bvh(c, w, st, std::min(blocks(2*bound, kTraceBlock), c->persist_blocks)); launches++; }
-    if (prof) cudaEventRecord(w.ev_k[slot][5], st);
-    k_accum<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, nxt, w.sr, bi, w.ctl, w.bin_keys, w.bin_hist); launches++;
-    if (prof) cudaEventRecord(w.ev_k[slot][6], st);
+    launches += enqueue_bounce(c, w, pb, nxt, st, bi, bound, prof ? &w.ev_k[slot][2] : nullptr);
     k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, has_bvh ? 1 : 0); launches++;
     if (has_bvh) { k_bin_scatter<<<blocks(bound, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order); launches++; }
     if (prof) cudaEventRecord(w.ev_k[slot][7], st);
@@ -924,6 +943,90 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const Batc
     return TGB_OK;
 }
 
+int single_render_resident(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed, uint32_t spp_begin, uint32_t spp_count) {
+    CU(cudaSetDevice(c->device));
+    int rc = set_tiles(c, tiles, n_tiles, seed);
+    if (rc) return rc;
+    return render_device(c, spp_begin, spp_count);
+}
+
+int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed, tgb_sample_record *records) {
+    static_assert(sizeof(tgb_sample_record) == sizeof(SampleRecordD), "record layout");
+    CU(cudaSetDevice(c->device));
+    int rc = set_tiles(c, tiles, n_tiles, seed);
+    if (rc) return rc;
+    const uint32_t var_w = (c->res_x + 3)/4, var_h = (c->res_y + 3)/4, n_blocks = var_w*var_h;
+    if (c->n_pix == 0) return TGB_OK;
+    std::vector<uint32_t> cnt(c->n_pix), base(size_t(c->n_pix) + 1, 0);
+    for (uint32_t i = 0; i < c->n_pix; ++i) {
+        const uint32_t px = c->h_pix_id[i] % c->res_x, py = c->h_pix_id[i]/c->res_x;
+        const tgb_sample_record &r = records[px/4 + (py/4)*var_w];
+        cnt[i] = r.next_sample_count; base[i] = r.sample_index;
+    }
+    // The step renders in runs of consecutive tiles of the list (the list is tile-major: a run is a range of c->pix_id), one
+    // pass each: at most kPassPaths paths, and every pixel's count fits the run's path ids.  A 4x4 block lies inside one
+    // tile, so its samples fold in one run, in renderTile's order, and the image and records do not depend on the runs.
+    struct Run { uint32_t p0, n, max_cnt; uint64_t total; };
+    const auto one_pass = [](uint32_t n, uint64_t total, uint32_t max_cnt) {
+        return total <= kPassPaths && uint64_t(max_cnt) <= (uint64_t(1) << (32 - index_bits(n)));
+    };
+    std::vector<Run> runs;
+    uint64_t step_total = 0;
+    for (uint32_t t = 0, p = 0; t < c->tiles_cached.size(); ++t) {
+        const tgb_tile &tl = c->tiles_cached[t];
+        const uint32_t n = tl.w*tl.h;
+        if (n == 0) continue;
+        uint64_t total = 0; uint32_t max_cnt = 0;
+        for (uint32_t i = p; i < p + n; ++i) { total += cnt[i]; max_cnt = std::max(max_cnt, cnt[i]); }
+        if (!one_pass(n, total, max_cnt))
+            return fail(c, TGB_ERR_UNSUPPORTED, "adaptive step: tile %u at (%u, %u) renders %llu paths, %u for one pixel: more than one pass holds",
+                        t, tl.x, tl.y, (unsigned long long)total, max_cnt);
+        if (runs.empty() || !one_pass(runs.back().n + n, runs.back().total + total, std::max(runs.back().max_cnt, max_cnt))) runs.push_back(Run{p, 0, 0, 0});
+        Run &r = runs.back();
+        r.n += n; r.total += total; r.max_cnt = std::max(r.max_cnt, max_cnt);
+        p += n; step_total += total;
+    }
+    // run k's result-slot offsets (n + 1 of them, from 0) start at pix_first[p0 + k]
+    std::vector<uint32_t> first(size_t(c->n_pix) + runs.size());
+    for (size_t k = 0; k < runs.size(); ++k) {
+        uint32_t *f = first.data() + runs[k].p0 + k, slot = 0;
+        for (uint32_t i = 0; i < runs[k].n; ++i) { f[i] = slot; slot += cnt[runs[k].p0 + i]; }
+        f[runs[k].n] = slot;
+    }
+    if (c->adaptive_capacity < first.size() || !c->rec_dev) {
+        if ((rc = dev_alloc(c, &c->pix_first, first.size()))) return rc;
+        if ((rc = dev_alloc(c, &c->pix_base, first.size()))) return rc;
+        if (!c->pix_slot && (rc = dev_alloc(c, &c->pix_slot, size_t(c->res_x)*c->res_y))) return rc;
+        if (!c->rec_dev && (rc = dev_alloc(c, &c->rec_dev, n_blocks))) return rc;
+        c->adaptive_capacity = uint32_t(first.size());
+    }
+    if (!c->pix_slot_valid) {
+        std::vector<uint32_t> slot(size_t(c->res_x)*c->res_y, 0xFFFFFFFFu);
+        for (uint32_t i = 0; i < c->n_pix; ++i) slot[c->h_pix_id[i]] = i;
+        CU(cudaMemcpyAsync(c->pix_slot, slot.data(), slot.size()*4, cudaMemcpyHostToDevice, c->stream));
+        CU(cudaStreamSynchronize(c->stream));
+        c->pix_slot_valid = true;
+    }
+    CU(cudaMemcpyAsync(c->pix_first, first.data(), first.size()*4, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(c->pix_base, base.data(), base.size()*4, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(c->rec_dev, records, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyHostToDevice, c->stream));
+    CU(cudaStreamSynchronize(c->stream));                       // (the host vectors go out of scope)
+    if (step_total == 0) return TGB_OK;
+    for (size_t k = 0; k < runs.size(); ++k) {
+        const Run &r = runs[k];
+        if (r.total == 0) continue;
+        BatchInfo bi; bi.pix_id = c->pix_id + r.p0; bi.pix_seed = c->pix_seed + r.p0; bi.n_pix = r.n; bi.spp_begin = 0;
+        bi.pix_first = c->pix_first + r.p0 + k; bi.pix_base = c->pix_base + r.p0; bi.pix_bits = index_bits(r.n);
+        if ((rc = render_device(c, 0, 0, &bi, uint32_t(r.total)))) return rc;
+        k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R, bi, c->pix_slot, r.p0, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
+        c->stats.kernel_launches++;
+    }
+    CU(cudaMemcpyAsync(records, c->rec_dev, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    CU(cudaGetLastError());
+    return TGB_OK;
+}
+
 // apply f to every member of a multi-GPU context (the root last, so that the current device ends up being the root's)
 template <class F> int for_members(tgb_ctx *c, F f) {
     if (!c->group) return TGB_OK;
@@ -943,29 +1046,23 @@ void shard_order(const tgb_tile *tiles, uint32_t n, std::vector<uint32_t> &order
     std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return morton2(tiles[a].x/16u, tiles[a].y/16u) < morton2(tiles[b].x/16u, tiles[b].y/16u); });
 }
 
-int single_render_resident(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed, uint32_t spp_begin, uint32_t spp_count);
-int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed, tgb_sample_record *records);
-
 // Deal the call's tiles to the members (Morton order, round-robin) and make sure the root knows every share's pixel list.
 int group_deal(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed) {
     tgb_ctx *c = root; Group &g = *root->group;
-    std::vector<tgb_tile> own;
-    if (n_tiles == 0) { dice_tiles(root->res_x, root->res_y, seed, own); tiles = own.data(); n_tiles = uint32_t(own.size()); }
-    if (g.deal_key.size() == n_tiles && n_tiles && std::memcmp(g.deal_key.data(), tiles, n_tiles*sizeof(tgb_tile)) == 0) return TGB_OK;
+    std::vector<tgb_tile> list = call_tiles(root, tiles, n_tiles, seed);
+    if (same_tiles(list, g.deal_key)) return TGB_OK;
+    std::vector<uint32_t> pid;
+    if (int rc = tile_pixels(root, list, pid)) return rc;     // the whole list: no pixel is rendered by two members
     const size_t N = g.members.size();
-    std::vector<uint32_t> order; shard_order(tiles, n_tiles, order);
+    std::vector<uint32_t> order; shard_order(list.data(), uint32_t(list.size()), order);
     g.shares.assign(N, {});
-    for (uint32_t i = 0; i < n_tiles; ++i) g.shares[i % N].push_back(tiles[order[i]]);
+    for (uint32_t i = 0; i < list.size(); ++i) g.shares[i % N].push_back(list[order[i]]);
     CU(cudaSetDevice(root->device));
     for (uint32_t *p : g.root_pix) if (p) cudaFree(p);
     g.root_pix.assign(N, nullptr); g.share_pixels.assign(N, 0);
     size_t max_share = 0;
     for (size_t k = 0; k < N; ++k) {
-        std::vector<uint32_t> pid;
-        for (const tgb_tile &tl : g.shares[k]) {
-            if (tl.x >= root->res_x || tl.w > root->res_x - tl.x || tl.y >= root->res_y || tl.h > root->res_y - tl.y) return fail(c, TGB_ERR_INVALID, "tile lies outside the image");
-            for (uint32_t y = 0; y < tl.h; ++y) for (uint32_t x = 0; x < tl.w; ++x) pid.push_back((tl.x + x) + (tl.y + y)*root->res_x);
-        }
+        if (int rc = tile_pixels(root, g.shares[k], pid)) return rc;
         g.share_pixels[k] = uint32_t(pid.size());
         max_share = std::max(max_share, pid.size());
         if (k >= 1 && !pid.empty()) {
@@ -990,7 +1087,7 @@ int group_deal(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_t 
             g.send_capacity[k] = g.share_pixels[k];
         }
     }
-    g.deal_key.assign(tiles, tiles + n_tiles); g.deal_seed = seed;
+    g.deal_key = std::move(list);
     return TGB_OK;
 }
 
@@ -1050,6 +1147,192 @@ int group_render(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_
     return TGB_OK;
 }
 
+int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
+    tgb_ctx *c = nullptr;
+    *out = nullptr;
+    if (d->abi_version != TGB200_ABI_VERSION) return fail(nullptr, TGB_ERR_INVALID, "ABI version mismatch (got %u, library is %u)", d->abi_version, TGB200_ABI_VERSION);
+    if (!d->settings.use_sobol) return fail(nullptr, TGB_ERR_UNSUPPORTED, "only the Sobol sampler (renderer.stratified_sampler = true) is on the hot path");
+    if (d->settings.supplemental_mode != 0) return fail(nullptr, TGB_ERR_UNSUPPORTED, "supplemental_mode %u: the per-tile serial PCG stream cannot be reproduced by a wavefront renderer (DESIGN.md section 3)", d->settings.supplemental_mode);
+    if (d->camera.res_x == 0 || d->camera.res_y == 0) return fail(nullptr, TGB_ERR_INVALID, "empty image");
+    // max_bounces 0: PathTracer::traceSample's loop never runs and every sample is black; the wavefront's first shade would add
+    // bounce-0 emission, so the setting is refused rather than rendered differently
+    if (d->settings.max_bounces > 255 || d->settings.max_bounces < 1) return fail(nullptr, TGB_ERR_UNSUPPORTED, "max_bounces must be in [1, 255]");
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(nullptr, TGB_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU fallback)"); }
+    int dev = d->settings.device;
+    if (dev < 0) { if (cudaGetDevice(&dev) != cudaSuccess) dev = 0; }
+    if (dev >= ndev) return fail(nullptr, TGB_ERR_NO_DEVICE, "CUDA device %d not present (%d devices)", dev, ndev);
+    cudaDeviceProp prop;
+    if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(nullptr, TGB_ERR_NO_DEVICE, "cannot query device %d", dev);
+    if (prop.major != 9 || prop.minor != 0) return fail(nullptr, TGB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major, prop.minor);
+    c = new tgb_ctx();
+    c->device = dev;
+    int rc = TGB_OK;
+    do {
+        if (cudaSetDevice(dev) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", dev); break; }
+        if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
+            cudaStreamCreateWithFlags(&c->stream1, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaStreamCreate failed"); break; }
+        c->stream = c->own_stream;
+        for (cudaEvent_t *e : {&c->ev0, &c->ev1}) cudaEventCreate(e);
+        for (cudaEvent_t *e : {&c->ev_fork, &c->ev_join}) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
+        for (Wavefront &w : c->wf)
+            for (int k = 0; k < 4; ++k) {
+                cudaEventCreateWithFlags(&w.ev_ring[k], cudaEventDisableTiming);
+                for (cudaEvent_t &e : w.ev_k[k]) cudaEventCreate(&e);
+            }
+        if ((rc = upload_scene(c, d))) break;
+        c->ks = select_kernels(c);
+        // default: 2 x 4 Mi paths in flight (H100, C1: 2 x 2 Mi measured 3 % slower)
+        uint32_t cap = d->settings.max_paths_in_flight ? d->settings.max_paths_in_flight : (1u << 23);
+        cap = std::max(cap, 1024u);
+        if ((rc = alloc_wavefront(c, cap))) break;
+        {   // persistent traversal grid of one wavefront: what is resident at once (blocks per SM x SMs, smaller of the two
+            // kernels), or TGB_TRAVERSAL_BLOCKS per SM.  H100, C1: 6 (resident) > 4 > 12 (twice resident) > 3 blocks per SM.
+            int sms = 0, b1 = 0, b2 = 0;
+            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+            cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, c->ks.trace, kTraceBlock, 0);
+            if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b2, c->ks.shadow_bvh, kTraceBlock, 0);
+            if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
+            const char *per_sm = getenv("TGB_TRAVERSAL_BLOCKS");
+            c->persist_blocks = uint32_t(sms)*uint32_t(per_sm ? std::max(1, atoi(per_sm)) : std::min(b1, b2));
+        }
+    } while (0);
+    if (rc) { g_create_error = c->error; tgb200_destroy(c); return rc; }
+    *out = c;
+    return TGB_OK;
+}
+
+// Closest hits of n device rays through the analytic pass and the renderer's traversal kernels (into device Hit records)
+// As in a render, rays that miss the BVH's top-level cut before their analytic hit skip the traversal (TGB_HOOK_CUT=0: every ray
+// is traversed).
+cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t n) {
+    const char *cut_env = getenv("TGB_HOOK_CUT");
+    const int cut = (cut_env && cut_env[0] == '0') ? 0 : 1;
+    uint32_t *list = nullptr;                                   // [count | indices of the rays to traverse]
+    cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&list), (size_t(n) + 1)*sizeof(uint32_t), c->stream);
+    if (e != cudaSuccess) return e;
+    e = cudaMemsetAsync(list, 0, sizeof(uint32_t), c->stream);
+    if (e == cudaSuccess) {
+        k_hook_analytic<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, n, cut, list + 1, list);
+        c->stats.kernel_launches++;
+    }
+    if (e == cudaSuccess && c->sc.n_nodes) {
+        // the renderer's own persistent kernel body (lane refill)
+        uint32_t *cursor = &c->wf[0].ctl->cursor_trace;
+        e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), c->stream);
+        uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
+        if (e == cudaSuccess) c->ks.hook_persist<<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, cursor);
+        c->stats.kernel_launches++;
+    }
+    const cudaError_t ef = cudaFreeAsync(list, c->stream);
+    return e != cudaSuccess ? e : ef;
+}
+
+// the pixel list of tgb200_pack_tiles / tgb200_unpack_tiles on the device (owned: a copy the caller frees)
+int device_tile_pixels(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t **dev, uint32_t *n_out, bool *owned) {
+    *owned = true;
+    const std::vector<tgb_tile> list(tiles, tiles + n_tiles);
+    if (same_tiles(list, c->tiles_cached)) {
+        *dev = c->pix_id; *n_out = c->n_pix; *owned = false;      // same tile list as the last render: reuse its pixel list
+        return TGB_OK;
+    }
+    std::vector<uint32_t> pid;
+    if (int rc = tile_pixels(c, list, pid)) return rc;
+    *n_out = uint32_t(pid.size()); *dev = nullptr;
+    if (pid.empty()) return TGB_OK;
+    CU(cudaMalloc(reinterpret_cast<void **>(dev), pid.size()*4));
+    cudaError_t e = cudaMemcpyAsync(*dev, pid.data(), pid.size()*4, cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e != cudaSuccess) { cudaFree(*dev); *dev = nullptr; return fail(c, TGB_ERR_CUDA, "tile upload failed: %s", cudaGetErrorString(e)); }
+    return TGB_OK;
+}
+
+// UniformSampler (sampling/UniformSampler.hpp:40-52): the integrator's own PCG32 stream (tile seeds, adaptive distribution)
+inline float pcg_next1d(uint64_t &state) { return normalized_uint(pcg_next(state)); }
+// Tungsten's min / max (math/MathUtil.hpp:10-26): a < b ? a : b and a > b ? a : b.  They agree with std::min / std::max on
+// numbers but not on NaN: a block whose mean overflowed to Inf has a NaN error estimate, and min(NaN, maxError) = maxError
+// gives it the largest weight, where std::min would carry the NaN into the dilation and the sample budget.
+inline float tungsten_min(float a, float b) { return a < b ? a : b; }
+inline float tungsten_max(float a, float b) { return a > b ? a : b; }
+
+// The tree tgb200_create builds for a scene of n triangles (9 floats each: v0 v1 v2) and nothing else.  extent = the largest
+// coordinate magnitude in play besides the triangles' (tgb200_create: the camera position's).
+void build_triangle_scene_bvh(const float *tri_verts, uint32_t n, float extent, SceneBvh &sb) {
+    std::vector<BuildTri> tris(n);
+    for (uint32_t i = 0; i < n; ++i) std::memcpy(&tris[i], tri_verts + 9*size_t(i), sizeof(BuildTri));
+    SceneBvhInput in;
+    in.tris = tris.data(); in.n_tris = n; in.extent = extent;
+    build_scene_bvh(in, bvh_options(), sb);
+}
+// 1/d as the kernels compute it: components no larger than 1e-30 in magnitude are replaced by +-1e-30
+void host_inv_dir(const V3 &d, float inv[3]) {
+    const float ooeps = 1e-30f;
+    inv[0] = 1.0f/(std::fabs(d.x) > ooeps ? d.x : std::copysign(ooeps, d.x));
+    inv[1] = 1.0f/(std::fabs(d.y) > ooeps ? d.y : std::copysign(ooeps, d.y));
+    inv[2] = 1.0f/(std::fabs(d.z) > ooeps ? d.z : std::copysign(ooeps, d.z));
+}
+// Traversal::triangle on the host, on the intersection record the kernels read: best = t when the triangle is hit in (tnear, best)
+bool host_triangle(const IsectRecord &rec, const V3 &o, const V3 &d, float tnear, float &best) {
+    const V3 v0 = f3(rec.f), e1 = f3(rec.f + 3), e2 = f3(rec.f + 6), ng = f3(rec.f + 9);
+    V3 C = v0 - o, R = cross(d, C);
+    auto edot = [](V3 a, V3 b) { return a.x*b.x + (a.y*b.y + a.z*b.z); };
+    float den = edot(ng, d), absDen = std::fabs(den);
+    auto xs = [&](float a) { return den < 0.0f || (den == 0.0f && std::signbit(den)) ? -a : a; };
+    float U = xs(edot(R, e2)), V = xs(edot(R, e1));
+    if (!(den != 0.0f && U >= 0.0f && V >= 0.0f && U + V <= absDen)) return false;
+    float T = xs(edot(ng, C));
+    if (!(T > absDen*tnear && T < absDen*best)) return false;
+    best = T/absDen;
+    return true;
+}
+
+// ---- test hooks: host arrays in, one probe kernel on the context's stream, host arrays out ----
+struct ProbeBufs {                  // device copies of a probe's arrays, freed on every exit
+    tgb_ctx *c; std::vector<void *> p;
+    Ctl *ctl_saved = nullptr; Counters *ctr_saved = nullptr; bool saved = false;
+    explicit ProbeBufs(tgb_ctx *ctx) : c(ctx) {}
+    ~ProbeBufs() { for (void *q : p) cudaFree(q); }
+    template <typename T> cudaError_t alloc(T **out, size_t n) {
+        void *q = nullptr;
+        cudaError_t e = cudaMalloc(&q, std::max<size_t>(n, 1)*sizeof(T));
+        if (e == cudaSuccess) p.push_back(q);
+        *out = static_cast<T *>(q);
+        return e;
+    }
+    template <typename T> cudaError_t upload(T **out, const T *src, size_t n) {
+        cudaError_t e = alloc(out, n);
+        return e != cudaSuccess ? e : cudaMemcpyAsync(*out, src, n*sizeof(T), cudaMemcpyHostToDevice, c->stream);
+    }
+    template <typename T> cudaError_t download(T *dst, const T *src, size_t n) {
+        return cudaMemcpyAsync(dst, src, n*sizeof(T), cudaMemcpyDeviceToHost, c->stream);
+    }
+    // Snapshot of wavefront 0's control block and the context's counters, which a probe that runs the renderer's kernels uses:
+    // its launches must not show in them or in the next render's statistics.  finish() queues the restore.
+    cudaError_t save_state() {
+        cudaError_t e = alloc(&ctl_saved, 1);
+        if (e == cudaSuccess) e = alloc(&ctr_saved, 1);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, c->wf[0].ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
+        saved = e == cudaSuccess;
+        return e;
+    }
+    int finish(cudaError_t e, const char *what) {
+        if (saved) {        // also when a launch failed: the copies are queued after whatever was queued
+            const cudaError_t r1 = cudaMemcpyAsync(c->wf[0].ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+            const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
+            if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
+        }
+        if (e == cudaSuccess) e = cudaGetLastError();
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        return e == cudaSuccess ? TGB_OK : fail(c, TGB_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
+    }
+};
+// lobe_set 1 (the Lambert-only instantiation) exists only without curves, as in k_shade
+int probe_check(tgb_ctx *c, int lobe_set) {
+    if (lobe_set != 0 && lobe_set != 1) return fail(c, TGB_ERR_INVALID, "lobe_set must be 0 or 1");
+    if (lobe_set == 1 && c->has_curves) return fail(c, TGB_ERR_INVALID, "lobe_set 1 has no instantiation with curves");
+    return TGB_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1089,8 +1372,6 @@ void tgb200_destroy(tgb_ctx *c) {
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;
 }
-
-static int create_single(const tgb_scene_desc *d, tgb_ctx **out);
 
 int tgb200_create(const tgb_scene_desc *d, tgb_ctx **out) {
     if (!d || !out) return fail(nullptr, TGB_ERR_INVALID, "null argument");
@@ -1132,64 +1413,6 @@ int tgb200_create(const tgb_scene_desc *d, tgb_ctx **out) {
     return TGB_OK;
 }
 
-static int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
-    tgb_ctx *c = nullptr;
-    *out = nullptr;
-    if (d->abi_version != TGB200_ABI_VERSION) return fail(nullptr, TGB_ERR_INVALID, "ABI version mismatch (got %u, library is %u)", d->abi_version, TGB200_ABI_VERSION);
-    if (!d->settings.use_sobol) return fail(nullptr, TGB_ERR_UNSUPPORTED, "only the Sobol sampler (renderer.stratified_sampler = true) is on the hot path");
-    if (d->settings.supplemental_mode != 0) return fail(nullptr, TGB_ERR_UNSUPPORTED, "supplemental_mode %u: the per-tile serial PCG stream cannot be reproduced by a wavefront renderer (DESIGN.md section 3)", d->settings.supplemental_mode);
-    if (d->camera.res_x == 0 || d->camera.res_y == 0) return fail(nullptr, TGB_ERR_INVALID, "empty image");
-    // max_bounces 0: PathTracer::traceSample's loop never runs and every sample is black; the wavefront's first shade would add
-    // bounce-0 emission, so the setting is refused rather than rendered differently
-    if (d->settings.max_bounces > 255 || d->settings.max_bounces < 1) return fail(nullptr, TGB_ERR_UNSUPPORTED, "max_bounces must be in [1, 255]");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(nullptr, TGB_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU fallback)"); }
-    int dev = d->settings.device;
-    if (dev < 0) { if (cudaGetDevice(&dev) != cudaSuccess) dev = 0; }
-    if (dev >= ndev) return fail(nullptr, TGB_ERR_NO_DEVICE, "CUDA device %d not present (%d devices)", dev, ndev);
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(nullptr, TGB_ERR_NO_DEVICE, "cannot query device %d", dev);
-    if (prop.major != 9 || prop.minor != 0) return fail(nullptr, TGB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major, prop.minor);
-    c = new tgb_ctx();
-    c->device = dev;
-    int rc = TGB_OK;
-    do {
-        if (cudaSetDevice(dev) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", dev); break; }
-        if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaStreamCreateWithFlags(&c->stream1, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaStreamCreate failed"); break; }
-        c->stream = c->own_stream;
-        for (cudaEvent_t *e : {&c->ev0, &c->ev1}) cudaEventCreate(e);
-        for (cudaEvent_t *e : {&c->ev_fork, &c->ev_join}) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
-        for (Wavefront &w : c->wf)
-            for (int k = 0; k < 4; ++k) {
-                cudaEventCreateWithFlags(&w.ev_ring[k], cudaEventDisableTiming);
-                for (cudaEvent_t &e : w.ev_k[k]) cudaEventCreate(&e);
-            }
-        if ((rc = upload_scene(c, d))) break;
-        // default: 2 x 4 Mi paths in flight (H100, C1: 2 x 2 Mi measured 3 % slower)
-        uint32_t cap = d->settings.max_paths_in_flight ? d->settings.max_paths_in_flight : (1u << 23);
-        cap = std::max(cap, 1024u);
-        if ((rc = alloc_wavefront(c, cap))) break;
-        {   // persistent traversal grid of one wavefront: what is resident at once (blocks per SM x SMs, smaller of the two
-            // kernels), or TGB_TRAVERSAL_BLOCKS per SM.  H100, C1: 6 (resident) > 4 > 12 (twice resident) > 3 blocks per SM.
-            int sms = 0, b1 = 0, b2 = 0;
-            cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-            cudaError_t e = cudaSuccess;
-            auto prep = [&](auto kern, int *nb) {
-                if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(nb, kern, kTraceBlock, 0);
-            };
-            if (c->has_curves) { prep(k_trace<true>, &b1); prep(c->mesh_lights ? k_shadow_bvh<true, true> : k_shadow_bvh<true, false>, &b2); }
-            else { prep(k_trace<false>, &b1); prep(c->mesh_lights ? k_shadow_bvh<false, true> : k_shadow_bvh<false, false>, &b2); }
-            if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
-            const char *per_sm = getenv("TGB_TRAVERSAL_BLOCKS");
-            c->persist_blocks = uint32_t(sms)*uint32_t(per_sm ? std::max(1, atoi(per_sm)) : std::min(b1, b2));
-        }
-    } while (0);
-    if (rc) { g_create_error = c->error; tgb200_destroy(c); return rc; }
-    *out = c;
-    return TGB_OK;
-}
-
 int tgb200_clear_framebuffer(tgb_ctx *c) {
     if (!c) return TGB_ERR_INVALID;
     { int rc = for_members(c, [](tgb_ctx *m) { return tgb200_clear_framebuffer(m); }); if (rc) return rc; }
@@ -1207,16 +1430,6 @@ int tgb200_render_resident(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
     if (c->group) return group_render(c, tiles, n_tiles, seed, spp_begin, spp_count, nullptr);
     return single_render_resident(c, tiles, n_tiles, seed, spp_begin, spp_count);
 }
-}  // extern "C"
-namespace {
-int single_render_resident(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed, uint32_t spp_begin, uint32_t spp_count) {
-    CU(cudaSetDevice(c->device));
-    int rc = set_tiles(c, tiles, n_tiles, seed);
-    if (rc) return rc;
-    return render_device(c, spp_begin, spp_count);
-}
-}  // namespace
-extern "C" {
 
 int tgb200_read_framebuffer(tgb_ctx *c, float *rgb_mean, uint32_t *count) {
     if (!c || !rgb_mean) return TGB_ERR_INVALID;
@@ -1267,35 +1480,6 @@ int tgb200_framebuffer_device_ptr(tgb_ctx *c, void **rgb_mean_dev, uint64_t *n_b
     *rgb_mean_dev = c->fb;
     if (n_bytes) *n_bytes = uint64_t(c->res_x)*c->res_y*3*sizeof(float);
     return TGB_OK;
-}
-
-// Closest hits of n device rays through the analytic pass and the renderer's traversal kernels (into device Hit records)
-// As in a render, rays that miss the BVH's top-level cut before their analytic hit skip the traversal (TGB_HOOK_CUT=0: every ray
-// is traversed).
-static cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t n) {
-    const char *cut_env = getenv("TGB_HOOK_CUT");
-    const int cut = (cut_env && cut_env[0] == '0') ? 0 : 1;
-    uint32_t *list = nullptr;                                   // [count | indices of the rays to traverse]
-    cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&list), (size_t(n) + 1)*sizeof(uint32_t), c->stream);
-    if (e != cudaSuccess) return e;
-    e = cudaMemsetAsync(list, 0, sizeof(uint32_t), c->stream);
-    if (e == cudaSuccess) {
-        k_hook_analytic<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, n, cut, list + 1, list);
-        c->stats.kernel_launches++;
-    }
-    if (e == cudaSuccess && c->sc.n_nodes) {
-        // the renderer's own persistent kernel body (lane refill)
-        uint32_t *cursor = &c->wf[0].ctl->cursor_trace;
-        e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), c->stream);
-        uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
-        if (e == cudaSuccess) {
-            if (c->has_curves) k_hook_persist<true><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, cursor);
-            else k_hook_persist<false><<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, cursor);
-        }
-        c->stats.kernel_launches++;
-    }
-    const cudaError_t ef = cudaFreeAsync(list, c->stream);
-    return e != cudaSuccess ? e : ef;
 }
 
 int tgb200_trace_closest(tgb_ctx *c, const tgb_ray *rays, tgb_hit *hits, uint32_t n) {
@@ -1378,32 +1562,11 @@ int tgb200_scene_info(tgb_ctx *c, uint32_t *n_tris, uint32_t *n_nodes, uint32_t 
     return TGB_OK;
 }
 
-static int tile_pixels(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t **dev, uint32_t *n_out, bool *owned) {
-    *owned = true;
-    if (c->tiles_cached.size() == n_tiles && n_tiles && std::memcmp(c->tiles_cached.data(), tiles, n_tiles*sizeof(tgb_tile)) == 0) {
-        *dev = c->pix_id; *n_out = c->n_pix; *owned = false;      // same tile list as the last render: reuse its pixel list
-        return TGB_OK;
-    }
-    std::vector<uint32_t> pid;
-    for (uint32_t t = 0; t < n_tiles; ++t) {
-        const tgb_tile &tl = tiles[t];
-        if (tl.x >= c->res_x || tl.w > c->res_x - tl.x || tl.y >= c->res_y || tl.h > c->res_y - tl.y) return fail(c, TGB_ERR_INVALID, "tile %u lies outside the image", t);
-        for (uint32_t y = 0; y < tl.h; ++y) for (uint32_t x = 0; x < tl.w; ++x) pid.push_back((tl.x + x) + (tl.y + y)*c->res_x);
-    }
-    *n_out = uint32_t(pid.size()); *dev = nullptr;
-    if (pid.empty()) return TGB_OK;
-    CU(cudaMalloc(reinterpret_cast<void **>(dev), pid.size()*4));
-    cudaError_t e = cudaMemcpyAsync(*dev, pid.data(), pid.size()*4, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { cudaFree(*dev); *dev = nullptr; return fail(c, TGB_ERR_CUDA, "tile upload failed: %s", cudaGetErrorString(e)); }
-    return TGB_OK;
-}
-
 int tgb200_pack_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, void *rgb_out_dev) {
     if (!c || !tiles || !rgb_out_dev) return TGB_ERR_INVALID;
     CU(cudaSetDevice(c->device));
     uint32_t *pid = nullptr, n = 0; bool owned = true;
-    int rc = tile_pixels(c, tiles, n_tiles, &pid, &n, &owned);
+    int rc = device_tile_pixels(c, tiles, n_tiles, &pid, &n, &owned);
     if (rc || !n) return rc;
     k_pack_tiles<<<blocks(n, 256), 256, 0, c->stream>>>(pid, n, c->fb, static_cast<float *>(rgb_out_dev));
     c->stats.kernel_launches++;
@@ -1417,7 +1580,7 @@ int tgb200_unpack_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, con
     if (!c || !tiles || !rgb_in_dev) return TGB_ERR_INVALID;
     CU(cudaSetDevice(c->device));
     uint32_t *pid = nullptr, n = 0; bool owned = true;
-    int rc = tile_pixels(c, tiles, n_tiles, &pid, &n, &owned);
+    int rc = device_tile_pixels(c, tiles, n_tiles, &pid, &n, &owned);
     if (rc || !n) return rc;
     k_unpack_tiles<<<blocks(n, 256), 256, 0, c->stream>>>(pid, n, static_cast<const float *>(rgb_in_dev), c->fb, c->fb_count, sample_count);
     c->stats.kernel_launches++;
@@ -1509,102 +1672,12 @@ int tgb200_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
     if (c->group) return group_render(c, tiles, n_tiles, seed, 0, 0, records);
     return single_render_adaptive(c, tiles, n_tiles, seed, records);
 }
-}  // extern "C"
-namespace {
-int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed, tgb_sample_record *records) {
-    static_assert(sizeof(tgb_sample_record) == sizeof(SampleRecordD), "record layout");
-    CU(cudaSetDevice(c->device));
-    int rc = set_tiles(c, tiles, n_tiles, seed);
-    if (rc) return rc;
-    const uint32_t var_w = (c->res_x + 3)/4, var_h = (c->res_y + 3)/4, n_blocks = var_w*var_h;
-    if (c->n_pix == 0) return TGB_OK;
-    std::vector<uint32_t> cnt(c->n_pix), base(size_t(c->n_pix) + 1, 0);
-    for (uint32_t i = 0; i < c->n_pix; ++i) {
-        const uint32_t px = c->h_pix_id[i] % c->res_x, py = c->h_pix_id[i]/c->res_x;
-        const tgb_sample_record &r = records[px/4 + (py/4)*var_w];
-        cnt[i] = r.next_sample_count; base[i] = r.sample_index;
-    }
-    // The step renders in runs of consecutive tiles of the list (the list is tile-major: a run is a range of c->pix_id), one
-    // pass each: at most kPassPaths paths, and every pixel's count fits the run's path ids.  A 4x4 block lies inside one
-    // tile, so its samples fold in one run, in renderTile's order, and the image and records do not depend on the runs.
-    struct Run { uint32_t p0, n, max_cnt; uint64_t total; };
-    const auto one_pass = [](uint32_t n, uint64_t total, uint32_t max_cnt) {
-        return total <= kPassPaths && uint64_t(max_cnt) <= (uint64_t(1) << (32 - index_bits(n)));
-    };
-    std::vector<Run> runs;
-    uint64_t step_total = 0;
-    for (uint32_t t = 0, p = 0; t < c->tiles_cached.size(); ++t) {
-        const tgb_tile &tl = c->tiles_cached[t];
-        const uint32_t n = tl.w*tl.h;
-        if (n == 0) continue;
-        uint64_t total = 0; uint32_t max_cnt = 0;
-        for (uint32_t i = p; i < p + n; ++i) { total += cnt[i]; max_cnt = std::max(max_cnt, cnt[i]); }
-        if (!one_pass(n, total, max_cnt))
-            return fail(c, TGB_ERR_UNSUPPORTED, "adaptive step: tile %u at (%u, %u) renders %llu paths, %u for one pixel: more than one pass holds",
-                        t, tl.x, tl.y, (unsigned long long)total, max_cnt);
-        if (runs.empty() || !one_pass(runs.back().n + n, runs.back().total + total, std::max(runs.back().max_cnt, max_cnt))) runs.push_back(Run{p, 0, 0, 0});
-        Run &r = runs.back();
-        r.n += n; r.total += total; r.max_cnt = std::max(r.max_cnt, max_cnt);
-        p += n; step_total += total;
-    }
-    // run k's result-slot offsets (n + 1 of them, from 0) start at pix_first[p0 + k]
-    std::vector<uint32_t> first(size_t(c->n_pix) + runs.size());
-    for (size_t k = 0; k < runs.size(); ++k) {
-        uint32_t *f = first.data() + runs[k].p0 + k, slot = 0;
-        for (uint32_t i = 0; i < runs[k].n; ++i) { f[i] = slot; slot += cnt[runs[k].p0 + i]; }
-        f[runs[k].n] = slot;
-    }
-    if (c->adaptive_capacity < first.size() || !c->rec_dev) {
-        if ((rc = dev_alloc(c, &c->pix_first, first.size()))) return rc;
-        if ((rc = dev_alloc(c, &c->pix_base, first.size()))) return rc;
-        if (!c->pix_slot && (rc = dev_alloc(c, &c->pix_slot, size_t(c->res_x)*c->res_y))) return rc;
-        if (!c->rec_dev && (rc = dev_alloc(c, &c->rec_dev, n_blocks))) return rc;
-        c->adaptive_capacity = uint32_t(first.size());
-    }
-    if (!c->pix_slot_valid) {
-        std::vector<uint32_t> slot(size_t(c->res_x)*c->res_y, 0xFFFFFFFFu);
-        for (uint32_t i = 0; i < c->n_pix; ++i) slot[c->h_pix_id[i]] = i;
-        CU(cudaMemcpyAsync(c->pix_slot, slot.data(), slot.size()*4, cudaMemcpyHostToDevice, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
-        c->pix_slot_valid = true;
-    }
-    CU(cudaMemcpyAsync(c->pix_first, first.data(), first.size()*4, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->pix_base, base.data(), base.size()*4, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->rec_dev, records, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyHostToDevice, c->stream));
-    CU(cudaStreamSynchronize(c->stream));                       // (the host vectors go out of scope)
-    if (step_total == 0) return TGB_OK;
-    for (size_t k = 0; k < runs.size(); ++k) {
-        const Run &r = runs[k];
-        if (r.total == 0) continue;
-        BatchInfo bi; bi.pix_id = c->pix_id + r.p0; bi.pix_seed = c->pix_seed + r.p0; bi.n_pix = r.n; bi.spp_begin = 0;
-        bi.pix_first = c->pix_first + r.p0 + k; bi.pix_base = c->pix_base + r.p0; bi.pix_bits = index_bits(r.n);
-        if ((rc = render_device(c, 0, 0, &bi, uint32_t(r.total)))) return rc;
-        k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R, bi, c->pix_slot, r.p0, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
-        c->stats.kernel_launches++;
-    }
-    CU(cudaMemcpyAsync(records, c->rec_dev, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyDeviceToHost, c->stream));
-    CU(cudaStreamSynchronize(c->stream));
-    CU(cudaGetLastError());
-    return TGB_OK;
-}
-}  // namespace
-extern "C" {
 
 int tgb200_shard_tiles(const tgb_tile *tiles, uint32_t n_tiles, uint32_t *order) {
     if ((n_tiles && !tiles) || !order) return TGB_ERR_INVALID;
     std::vector<uint32_t> o; shard_order(tiles, n_tiles, o);
     std::memcpy(order, o.data(), size_t(n_tiles)*4);
     return TGB_OK;
-}
-
-namespace {
-// UniformSampler (sampling/UniformSampler.hpp:40-52): the integrator's own PCG32 stream (tile seeds, adaptive distribution)
-inline float pcg_next1d(uint64_t &state) { return normalized_uint(pcg_next(state)); }
-// Tungsten's min / max (math/MathUtil.hpp:10-26): a < b ? a : b and a > b ? a : b.  They agree with std::min / std::max on
-// numbers but not on NaN: a block whose mean overflowed to Inf has a NaN error estimate, and min(NaN, maxError) = maxError
-// gives it the largest weight, where std::min would carry the NaN into the dilation and the sample budget.
-inline float tungsten_min(float a, float b) { return a < b ? a : b; }
-inline float tungsten_max(float a, float b) { return a > b ? a : b; }
 }
 
 // PathTraceIntegrator::generateWork (PathTraceIntegrator.cpp:44-134), host only: advances every block's sample index, then
@@ -1662,39 +1735,6 @@ int tgb200_generate_work(tgb_sample_record *records, uint32_t res_x, uint32_t re
     }
     return 1;
 }
-
-namespace {
-// The tree tgb200_create builds for a scene of n triangles (9 floats each: v0 v1 v2) and nothing else.  extent = the largest
-// coordinate magnitude in play besides the triangles' (tgb200_create: the camera position's).
-void build_triangle_scene_bvh(const float *tri_verts, uint32_t n, float extent, SceneBvh &sb) {
-    std::vector<BuildTri> tris(n);
-    for (uint32_t i = 0; i < n; ++i) std::memcpy(&tris[i], tri_verts + 9*size_t(i), sizeof(BuildTri));
-    SceneBvhInput in;
-    in.tris = tris.data(); in.n_tris = n; in.extent = extent;
-    build_scene_bvh(in, bvh_options(), sb);
-}
-// 1/d as the kernels compute it: components no larger than 1e-30 in magnitude are replaced by +-1e-30
-void host_inv_dir(const V3 &d, float inv[3]) {
-    const float ooeps = 1e-30f;
-    inv[0] = 1.0f/(std::fabs(d.x) > ooeps ? d.x : std::copysign(ooeps, d.x));
-    inv[1] = 1.0f/(std::fabs(d.y) > ooeps ? d.y : std::copysign(ooeps, d.y));
-    inv[2] = 1.0f/(std::fabs(d.z) > ooeps ? d.z : std::copysign(ooeps, d.z));
-}
-// Traversal::triangle on the host, on the intersection record the kernels read: best = t when the triangle is hit in (tnear, best)
-bool host_triangle(const IsectRecord &rec, const V3 &o, const V3 &d, float tnear, float &best) {
-    const V3 v0 = f3(rec.f), e1 = f3(rec.f + 3), e2 = f3(rec.f + 6), ng = f3(rec.f + 9);
-    V3 C = v0 - o, R = cross(d, C);
-    auto edot = [](V3 a, V3 b) { return a.x*b.x + (a.y*b.y + a.z*b.z); };
-    float den = edot(ng, d), absDen = std::fabs(den);
-    auto xs = [&](float a) { return den < 0.0f || (den == 0.0f && std::signbit(den)) ? -a : a; };
-    float U = xs(edot(R, e2)), V = xs(edot(R, e1));
-    if (!(den != 0.0f && U >= 0.0f && V >= 0.0f && U + V <= absDen)) return false;
-    float T = xs(edot(ng, C));
-    if (!(T > absDen*tnear && T < absDen*best)) return false;
-    best = T/absDen;
-    return true;
-}
-}  // namespace
 
 // Host-only check of the quantised device BVH (no GPU needed): builds the tree tgb200_create builds for a scene of n triangles
 // (the rays' origins take the camera's part in the padding) and walks it on the HOST with the kernels' node arithmetic
@@ -1828,43 +1868,6 @@ int tgb200_shadow_walk_count(const float *tri_verts, uint32_t n, const float *ca
     return TGB_OK;
 }
 
-}  // extern "C"
-
-// ---- test hooks: host arrays in, one probe kernel on the context's stream, host arrays out ----
-namespace {
-struct ProbeBufs {                  // device copies of a probe's arrays, freed on every exit
-    tgb_ctx *c; std::vector<void *> p;
-    explicit ProbeBufs(tgb_ctx *ctx) : c(ctx) {}
-    ~ProbeBufs() { for (void *q : p) cudaFree(q); }
-    template <typename T> cudaError_t alloc(T **out, size_t n) {
-        void *q = nullptr;
-        cudaError_t e = cudaMalloc(&q, std::max<size_t>(n, 1)*sizeof(T));
-        if (e == cudaSuccess) p.push_back(q);
-        *out = static_cast<T *>(q);
-        return e;
-    }
-    template <typename T> cudaError_t upload(T **out, const T *src, size_t n) {
-        cudaError_t e = alloc(out, n);
-        return e != cudaSuccess ? e : cudaMemcpyAsync(*out, src, n*sizeof(T), cudaMemcpyHostToDevice, c->stream);
-    }
-    template <typename T> cudaError_t download(T *dst, const T *src, size_t n) {
-        return cudaMemcpyAsync(dst, src, n*sizeof(T), cudaMemcpyDeviceToHost, c->stream);
-    }
-    int finish(cudaError_t e, const char *what) {
-        if (e == cudaSuccess) e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-        return e == cudaSuccess ? TGB_OK : fail(c, TGB_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
-    }
-};
-// lobe_set 1 (the Lambert-only instantiation) exists only without curves, as in k_shade
-int probe_check(tgb_ctx *c, int lobe_set) {
-    if (lobe_set != 0 && lobe_set != 1) return fail(c, TGB_ERR_INVALID, "lobe_set must be 0 or 1");
-    if (lobe_set == 1 && c->has_curves) return fail(c, TGB_ERR_INVALID, "lobe_set 1 has no instantiation with curves");
-    return TGB_OK;
-}
-}  // namespace
-
-extern "C" {
 
 int tgb200_bsdf_probe(tgb_ctx *c, int bsdf, float u, float v, uint32_t requested, int lobe_set, uint32_t n, const float *wi_wo,
                       float *out) {
@@ -1958,18 +1961,13 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    float *dq = nullptr, *dout = nullptr; int *dl = nullptr; Ctl *ctl_saved = nullptr; Counters *ctr_saved = nullptr;
+    float *dq = nullptr, *dout = nullptr; int *dl = nullptr;
     cudaError_t e = b.upload(&dq, query, 8*size_t(n));
     if (e == cudaSuccess) e = b.upload(&dl, light_mis, 2*size_t(n));
     if (e == cudaSuccess) e = b.alloc(&dout, 8*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&ctl_saved, 1);
-    if (e == cudaSuccess) e = b.alloc(&ctr_saved, 1);
-    // the probe's queries must not show in the context's control block or in the next render's statistics
+    if (e == cudaSuccess) e = b.save_state();
     const Wavefront &w = c->wf[0];
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, w.ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
-    const bool saved = e == cudaSuccess;
-    const DScene &sc = c->sc; const bool curves = c->has_curves; cudaStream_t st = c->stream;
+    const DScene &sc = c->sc; cudaStream_t st = c->stream;
     // one scratch slot per query: chunks of wavefront 0's capacity
     for (uint32_t off = 0; off < n && e == cudaSuccess; off += w.capacity) {
         const uint32_t m = std::min(w.capacity, n - off);
@@ -1978,18 +1976,12 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
         if (e != cudaSuccess) break;
         k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, w.sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
                                                             w.squeue, w.ctl, m);
-        if (curves) k_shadow_prep<true><<<blocks(m, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
-        else k_shadow_prep<false><<<blocks(m, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+        c->ks.shadow_prep<<<blocks(m, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
         k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(w.squeue2, w.squeue_cl, w.ctl, dout + 8*size_t(off));
-        if (sc.n_nodes) launch_shadow_bvh(c, w, st, std::min(blocks(m, kTraceBlock), c->persist_blocks));
+        if (sc.n_nodes)
+            c->ks.shadow_bvh<<<std::min(blocks(m, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
         k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(w.sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
         e = cudaGetLastError();
-    }
-    // restored also when a launch failed (the copies are queued after whatever was queued)
-    if (saved) {
-        const cudaError_t r1 = cudaMemcpyAsync(w.ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, st);
-        const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, st);
-        if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
     }
     if (e == cudaSuccess) e = b.download(out, dout, 8*size_t(n));
     return b.finish(e, "shadow_probe");
@@ -2009,16 +2001,11 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
     Wavefront &w = c->wf[0];
     if (int rc = ensure_results(c, w.capacity)) return rc;
     ProbeBufs b(c);
-    uint32_t *din = nullptr, *dout = nullptr, *pix = nullptr; Ctl *ctl_saved = nullptr; Counters *ctr_saved = nullptr;
+    uint32_t *din = nullptr, *dout = nullptr, *pix = nullptr;
     cudaError_t e = b.upload(&din, state_in, TGB_BOUNCE_WORDS*size_t(n));
     if (e == cudaSuccess) e = b.alloc(&dout, TGB_BOUNCE_WORDS*size_t(n));
     if (e == cudaSuccess) e = b.alloc(&pix, 4*size_t(w.capacity) + 1);
-    if (e == cudaSuccess) e = b.alloc(&ctl_saved, 1);
-    if (e == cudaSuccess) e = b.alloc(&ctr_saved, 1);
-    // the probe's paths must not show in the context's control block or in the next render's statistics
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, w.ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
-    const bool saved = e == cudaSuccess;
+    if (e == cudaSuccess) e = b.save_state();
     const DScene &sc = c->sc; cudaStream_t st = c->stream;
     PathBuf &pb = w.pb[0], &dst = w.pb[1];
     // per chunk: one pixel per path (pix_id, pix_seed, pix_first (m + 1 offsets), pix_base), so path id = result slot = its index
@@ -2034,30 +2021,18 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
         if (e != cudaSuccess) break;
         BatchInfo bi; bi.pix_id = pix_id; bi.pix_seed = pix_seed; bi.n_pix = m; bi.spp_begin = 0;
         bi.pix_first = pix_first; bi.pix_base = pix_base;
-        bi.pix_bits = 0; while ((1u << bi.pix_bits) < m) ++bi.pix_bits;
+        bi.pix_bits = index_bits(m);
         uint32_t *o = dout + TGB_BOUNCE_WORDS*size_t(off);
         k_probe_bounce_setup<<<blocks(m, 256), 256, 0, st>>>(sc, pb, din + TGB_BOUNCE_WORDS*size_t(off), pix_id, pix_seed, pix_first,
                                                             pix_base, w.bin_keys, w.bin_hist, o, m);
         k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, sc.n_nodes ? 1 : 0);
-        if (sc.n_nodes) {
-            k_bin_scatter<<<blocks(m, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
-            launch_trace(c, w, pb, st, m);
-        }
-        launch_shade(c, w, pb, st, bi, m);
-        launch_shadow_prep(c, w, st, m);
-        if (sc.n_nodes) launch_shadow_bvh(c, w, st, std::min(blocks(2*m, kTraceBlock), c->persist_blocks));
-        k_accum<<<blocks(m, 256), 256, 0, st>>>(sc, pb, dst, w.sr, bi, w.ctl, w.bin_keys, w.bin_hist);
+        if (sc.n_nodes) k_bin_scatter<<<blocks(m, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
+        enqueue_bounce(c, w, pb, dst, st, bi, m, nullptr);
         k_probe_bounce_alive<<<blocks(m, 256), 256, 0, st>>>(dst, w.ctl, o);
         k_probe_bounce_finished<<<blocks(m, 256), 256, 0, st>>>(pb, c->R, o, m);
         e = cudaGetLastError();
         // (the next chunk's control block is copied from this host variable: wait until this one is consumed)
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    }
-    // restored also when a launch failed (the copies are queued after whatever was queued)
-    if (saved) {
-        const cudaError_t r1 = cudaMemcpyAsync(w.ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, st);
-        const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, st);
-        if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
     }
     if (e == cudaSuccess) e = b.download(state_out, dout, TGB_BOUNCE_WORDS*size_t(n));
     return b.finish(e, "bounce_probe");
