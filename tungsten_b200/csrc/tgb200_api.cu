@@ -83,6 +83,7 @@ struct tgb_ctx {
     Wavefront wf[2];                // the hooks run on wf[0]'s buffers
     bool mesh_lights = false;       // a mesh is a light: closest-hit shadow queries exist, k_shadow_bvh<., false> runs
     uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels (per wavefront)
+    uint32_t regen_blocks = 0, prep_blocks = 0, scatter_blocks = 0;   // largest grids of the grid-stride kernels (resident blocks)
     bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
     bool quad_emitters = false;     // ... and only quad lights, constant textures: k_shade<.., .., 1, 1>
     bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
@@ -798,8 +799,8 @@ int ensure_results(tgb_ctx *c, size_t n_paths) {
 
 // One bounce of wavefront w's paths in pb on stream st: k_trace -> k_shade -> k_shadow_prep -> k_shadow_bvh -> k_accum (survivors
 // into nxt), as a render and tgb200_bounce_probe run it.  `bound` >= ctl.n: grids are upper bounds, the kernels read the real
-// sizes from the device-resident control block.  ev (profiling): events recorded after each of the five kernels.  Returns the
-// number of kernels launched.
+// sizes from the device-resident control block (k_shadow_prep loops over them with at most the resident blocks).  ev (profiling):
+// events recorded after each of the five kernels.  Returns the number of kernels launched.
 uint32_t enqueue_bounce(tgb_ctx *c, Wavefront &w, const PathBuf &pb, const PathBuf &nxt, cudaStream_t st, const BatchInfo &bi,
                         uint32_t bound, const cudaEvent_t *ev) {
     const DScene &sc = c->sc; const Kernels &ks = c->ks;
@@ -808,7 +809,7 @@ uint32_t enqueue_bounce(tgb_ctx *c, Wavefront &w, const PathBuf &pb, const PathB
     if (ev) cudaEventRecord(ev[0], st);
     ks.shade<<<blocks(bound, ks.shade_paths), ks.shade_block, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     if (ev) cudaEventRecord(ev[1], st);
-    ks.shadow_prep<<<blocks(2*bound, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+    ks.shadow_prep<<<std::min(blocks(2*bound, 256), c->prep_blocks), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
     if (ev) cudaEventRecord(ev[2], st);
     // the any-hit queue and (scenes with mesh lights) the closest-hit queue
     if (has_bvh) ks.shadow_bvh<<<std::min(blocks(2*bound, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
@@ -825,11 +826,11 @@ void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInf
     PathBuf &pb = w.pb[cur], &nxt = w.pb[cur ^ 1];
     const bool prof = c->profiling;
     if (prof) cudaEventRecord(w.ev_k[slot][0], st);
-    k_regen<<<blocks(bound, 256), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
+    k_regen<<<std::min(blocks(bound, 256), c->regen_blocks), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
     if (prof) cudaEventRecord(w.ev_k[slot][1], st);
     launches += enqueue_bounce(c, w, pb, nxt, st, bi, bound, prof ? &w.ev_k[slot][2] : nullptr);
     k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, has_bvh ? 1 : 0); launches++;
-    if (has_bvh) { k_bin_scatter<<<blocks(bound, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order); launches++; }
+    if (has_bvh) { k_bin_scatter<<<std::min(blocks(bound, 256), c->scatter_blocks), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order); launches++; }
     if (prof) cudaEventRecord(w.ev_k[slot][7], st);
 }
 
@@ -1195,6 +1196,14 @@ int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
             if (e != cudaSuccess || sms <= 0 || b1 <= 0 || b2 <= 0) { rc = fail(c, TGB_ERR_CUDA, "traversal kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
             const char *per_sm = getenv("TGB_TRAVERSAL_BLOCKS");
             c->persist_blocks = uint32_t(sms)*uint32_t(per_sm ? std::max(1, atoi(per_sm)) : std::min(b1, b2));
+            // k_regen, k_shadow_prep and k_bin_scatter loop over the device-side counts: a grid of what is resident at once
+            // instead of one sized for the worst case, whose blocks past the real count would only read ctl and exit
+            int br = 0, bp = 0, bs = 0;
+            e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&br, k_regen, 256, 0);
+            if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bp, c->ks.shadow_prep, 256, 0);
+            if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bs, k_bin_scatter, 256, 0);
+            if (e != cudaSuccess || br <= 0 || bp <= 0 || bs <= 0) { rc = fail(c, TGB_ERR_CUDA, "loop kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
+            c->regen_blocks = uint32_t(sms)*uint32_t(br); c->prep_blocks = uint32_t(sms)*uint32_t(bp); c->scatter_blocks = uint32_t(sms)*uint32_t(bs);
         }
     } while (0);
     if (rc) { g_create_error = c->error; tgb200_destroy(c); return rc; }

@@ -56,7 +56,8 @@ constexpr int HID_MISS = -1;
 struct Counters { unsigned long long rays, hits, shadow_rays, shadow_hits; };   // path queries / NEE+MIS queries
 
 // Device-resident control block of the wavefront loop.  k_iter_end writes the sizes of the NEXT iteration; every kernel of
-// an iteration reads them from here, its grid is only an upper bound chosen by the host from a snapshot one iteration old.
+// an iteration reads them from here, its grid is only an upper bound chosen by the host from a snapshot one iteration old (k_regen,
+// k_shadow_prep and k_bin_scatter loop over the sizes with at most the blocks that are resident at once).
 struct Ctl {
     uint32_t n;             // slots in use this iteration: survivors [0, n_surv) + new camera paths [n_surv, n)
     uint32_t n_surv;
@@ -821,12 +822,14 @@ TGB_D size_t path_result_slot(const BatchInfo &bi, uint32_t pix, uint32_t k) { r
 // slots are neighbouring pixels of one sample index, so the primary rays stay coherent and every state access is coalesced.
 // = SobolPathSampler::startPath + ReconstructionFilter::sample + PinholeCamera::sampleDirection + the analytic
 // part of the first TraceableScene::intersect.  Also clears the ray-coherence histogram for this iteration's k_accum.
+// The grid is what is resident at once (or less), each thread loops over the slots j, j + grid size, ...
 __global__ void __launch_bounds__(256) k_regen(DScene sc, PathBuf pb, BatchInfo bi, const Ctl *ctl, uint32_t *order, uint32_t *hist) {
-    const uint32_t j = blockIdx.x*blockDim.x + threadIdx.x;
-    for (uint32_t k = j; k < kBins; k += gridDim.x*blockDim.x) hist[k] = 0u;
-    if (j >= ctl->n_new) return;
-    const uint32_t i = ctl->n_surv + j;
-    const uint32_t path = ctl->first_path + j;
+    const uint32_t stride = gridDim.x*blockDim.x;
+    for (uint32_t k = blockIdx.x*blockDim.x + threadIdx.x; k < kBins; k += stride) hist[k] = 0u;
+    const uint32_t n_new = ctl->n_new, n_surv = ctl->n_surv, first_path = ctl->first_path;
+    for (uint32_t j = blockIdx.x*blockDim.x + threadIdx.x; j < n_new; j += stride) {
+    const uint32_t i = n_surv + j;
+    const uint32_t path = first_path + j;
     uint32_t pix, k;
     if (!bi.pix_first) { pix = path % bi.n_pix; k = path/bi.n_pix; }
     else {                                              // adaptive: the pixel whose result slots contain `path`
@@ -856,6 +859,7 @@ __global__ void __launch_bounds__(256) k_regen(DScene sc, PathBuf pb, BatchInfo 
     pb.E[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     pb.pcg[i] = smp.pcg;
     order[i] = i;                    // new camera paths are already coherent: visited in slot order, after the sorted survivors
+    }   // j
 }
 
 TGB_D void count_block(unsigned long long *rays, unsigned long long *hits, bool valid, bool hit) {
@@ -864,6 +868,56 @@ TGB_D void count_block(unsigned long long *rays, unsigned long long *hits, bool 
         atomicAdd(rays, (unsigned long long)__popc(mv));
         if (mh) atomicAdd(hits, (unsigned long long)__popc(mh));
     }
+}
+// The same for counts each thread has summed over the items it handled: reduced over the block in shared memory, one atomic
+// per counter and block.  Every thread of the block calls it.
+TGB_D void count_block_total(unsigned long long *rays, unsigned long long *hits, uint32_t n_rays, uint32_t n_hits) {
+    __shared__ uint32_t sum[2];
+    if (threadIdx.x == 0) { sum[0] = 0u; sum[1] = 0u; }
+    __syncthreads();
+    n_rays = __reduce_add_sync(0xffffffffu, n_rays); n_hits = __reduce_add_sync(0xffffffffu, n_hits);
+    if ((threadIdx.x & 31) == 0 && n_rays) { atomicAdd(&sum[0], n_rays); if (n_hits) atomicAdd(&sum[1], n_hits); }
+    __syncthreads();
+    if (threadIdx.x == 0 && sum[0]) {
+        atomicAdd(rays, (unsigned long long)sum[0]);
+        if (sum[1]) atomicAdd(hits, (unsigned long long)sum[1]);
+    }
+}
+// Queue allocation with one atomicAdd per block and queue: the lanes with take[q] set get consecutive entries of queue q, warp
+// after warp in block order (as per-warp allocations made in that order would hand them out).  Every thread of the block calls
+// it; at[q] is the lane's entry where take[q] is set.
+template <int Q, int BLOCK>
+TGB_D void block_alloc(uint32_t *const (&counter)[Q], const bool (&take)[Q], uint32_t (&at)[Q]) {
+    constexpr int WARPS = BLOCK/32;
+    static_assert(WARPS <= 32, "one warp scans the per-warp counts");
+    __shared__ uint32_t cnt[Q][WARPS];
+    const unsigned FULL = 0xffffffffu, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, lt = (1u << lane) - 1u;
+    unsigned m[Q];
+#pragma unroll
+    for (int q = 0; q < Q; ++q) m[q] = __ballot_sync(FULL, take[q]);
+    __syncthreads();                                            // a previous call's readers are done with cnt
+    if (lane == 0) {
+#pragma unroll
+        for (int q = 0; q < Q; ++q) cnt[q][warp] = __popc(m[q]);
+    }
+    __syncthreads();
+    if (warp == 0) {
+#pragma unroll
+        for (int q = 0; q < Q; ++q) {
+            const uint32_t c = lane < unsigned(WARPS) ? cnt[q][lane] : 0u;
+            uint32_t incl = c;
+#pragma unroll
+            for (uint32_t off = 1; off < unsigned(WARPS); off <<= 1) { const uint32_t v = __shfl_up_sync(FULL, incl, off); if (lane >= off) incl += v; }
+            const uint32_t total = __shfl_sync(FULL, incl, WARPS - 1);
+            uint32_t base = 0;
+            if (lane == 0 && total) base = atomicAdd(counter[q], total);
+            base = __shfl_sync(FULL, base, 0);
+            if (lane < unsigned(WARPS)) cnt[q][lane] = base + incl - c;
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < Q; ++q) at[q] = cnt[q][warp] + __popc(m[q] & lt);
 }
 
 // TraceableScene::intersect for the path rays: the analytic part of the query was done by the kernel that made the
@@ -1260,11 +1314,16 @@ k_shade(DScene sc, PathBuf pb, Scratch sr, BatchInfo bi, Ctl *ctl, uint32_t *squ
 // The queries left for the BVH are compacted into two queues, so that every warp of k_shadow_bvh runs one kind: any-hit queries
 // (quad / cap / environment lights) into squeue2 with the mask of the cut boxes they enter, closest-hit (mesh-light) queries into
 // squeue_cl with their analytic hit.
+// The grid is what is resident at once (or less): a block takes the runs of 256 queries [base, base + 256), base = its index
+// times 256 plus multiples of the grid's width, so every thread of a block makes the same number of trips (block_alloc).
 template <bool CURVES>
 __global__ void __launch_bounds__(256) k_shadow_prep(DScene sc, Scratch sr, const uint32_t *squeue, Ctl *ctl, uint32_t *squeue2,
                                                      uint32_t *squeue_cl, Counters *ctr) {
-    uint32_t i = blockIdx.x*blockDim.x + threadIdx.x;
-    bool valid = i < ctl->shadow_count;
+    const uint32_t n = ctl->shadow_count;
+    uint32_t n_valid = 0, n_blocked = 0;
+    for (uint32_t base = blockIdx.x*blockDim.x; base < n; base += gridDim.x*blockDim.x) {
+    const uint32_t i = base + threadIdx.x;
+    const bool valid = i < n;
     bool keep = false, blocked = false, any = false; uint32_t q = 0, cut = 0; Hit h; h.t = INFINITY; h.u = h.v = 0.0f; h.id = HID_MISS;
     if (valid) {
         q = squeue[i];
@@ -1282,28 +1341,22 @@ __global__ void __launch_bounds__(256) k_shadow_prep(DScene sc, Scratch sr, cons
             else keep = true;
         }
     }
-    count_block(&ctr->shadow_rays, &ctr->shadow_hits, valid, blocked);
-    const unsigned lane = threadIdx.x & 31, lt = (1u << lane) - 1u;
-    const unsigned ma = __ballot_sync(0xffffffffu, keep && any), mc = __ballot_sync(0xffffffffu, keep && !any);
-    if (ma) {
-        unsigned base = 0;
-        if (lane == 0) base = atomicAdd(&ctl->shadow_count2, unsigned(__popc(ma)));
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (keep && any) { const uint32_t at = base + __popc(ma & lt); squeue2[at] = q; sr.cut_mask[at] = cut; }
-    }
-    if (mc) {
-        unsigned base = 0;
-        if (lane == 0) base = atomicAdd(&ctl->shadow_count_closest, unsigned(__popc(mc)));
-        base = __shfl_sync(0xffffffffu, base, 0);
-        if (keep && !any) { const uint32_t at = base + __popc(mc & lt); squeue_cl[at] = q; sr.SH[at] = pack_hit(h); }
-    }
+    n_valid += valid ? 1u : 0u; n_blocked += blocked ? 1u : 0u;
+    uint32_t *const queue[2] = {&ctl->shadow_count2, &ctl->shadow_count_closest};
+    const bool take[2] = {keep && any, keep && !any};
+    uint32_t at[2];
+    block_alloc<2, 256>(queue, take, at);
+    if (take[0]) { squeue2[at[0]] = q; sr.cut_mask[at[0]] = cut; }
+    if (take[1]) { squeue_cl[at[1]] = q; sr.SH[at[1]] = pack_hit(h); }
+    }   // base
+    count_block_total(&ctr->shadow_rays, &ctr->shadow_hits, n_valid, n_blocked);
 }
 
 // ANY: the queue of any-hit queries (squeue2), else that of closest-hit queries (squeue_cl)
 template <bool CURVES, bool ANY>
 struct ShadowPolicy {
-    DScene sc; Scratch sr; const uint32_t *squeue; unsigned long long *hits;
-    uint32_t s, cut; bool mis; int li, ign; V3 p, d;
+    DScene sc; Scratch sr; const uint32_t *squeue;
+    uint32_t s, cut, blocked; bool mis; int li, ign; V3 p, d;      // blocked: the lane's queries that found a surface
     TGB_D bool fetch(uint32_t i, V3 &o, V3 &dd, float &tnear, Hit &h, bool &anyq) {
         uint32_t q = squeue[i];
         s = q >> 2; mis = q & 1u;
@@ -1328,7 +1381,7 @@ struct ShadowPolicy {
     }
     TGB_D int ignore() const { return ign; }
     TGB_D void finish(const Hit &h) {
-        if (h.id != HID_MISS) atomicAdd(hits, 1ull);
+        if (h.id != HID_MISS) blocked++;
         if (ANY) { if (h.id == HID_MISS) sr.vis[2*size_t(s) + (mis ? 1 : 0)] = 1u; }
         else shadow_resolve_closest<CURVES>(sc, sr, s, mis, li, p, d, h);
     }
@@ -1340,14 +1393,20 @@ template <bool CURVES, bool MESH_LIGHTS>
 __global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MINB) k_shadow_bvh(DScene sc, Scratch sr, const uint32_t *squeue2,
                                                                                                 const uint32_t *squeue_cl, Ctl *ctl, Counters *ctr) {
     __shared__ int smem_stack[kSmemStack*kTraceBlock];
+    uint32_t blocked;
     {
-        ShadowPolicy<CURVES, true> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue2; pol.hits = &ctr->shadow_hits;
+        ShadowPolicy<CURVES, true> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue2; pol.blocked = 0u;
         bvh_traverse_persistent<CURVES, true>(sc, smem_stack, pol, ctl->shadow_count2, &ctl->cursor_shadow);
+        blocked = pol.blocked;
     }
     if (MESH_LIGHTS) {
-        ShadowPolicy<CURVES, false> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue_cl; pol.hits = &ctr->shadow_hits;
+        ShadowPolicy<CURVES, false> pol; pol.sc = sc; pol.sr = sr; pol.squeue = squeue_cl; pol.blocked = blocked;
         bvh_traverse_persistent<CURVES, false>(sc, smem_stack, pol, ctl->shadow_count_closest, &ctl->cursor_closest);
+        blocked = pol.blocked;
     }
+    // every lane of the warp is here (the walks end when the whole warp is idle): one atomic per warp
+    blocked = __reduce_add_sync(0xffffffffu, blocked);
+    if ((threadIdx.x & 31) == 0 && blocked) atomicAdd(&ctr->shadow_hits, (unsigned long long)blocked);
 }
 
 // Fold this bounce's direct light + surface emission into the path (order as in handleSurface:537-543), apply the
@@ -1392,13 +1451,14 @@ __global__ void __launch_bounds__(256) k_accum(DScene sc, PathBuf pb, PathBuf ds
             sr.R[path_result_slot(bi, pix, k)] = make_float4(em.x, em.y, em.z, 0.0f);
         }
     }
-    unsigned m = __ballot_sync(0xffffffffu, alive);
-    if (m) {
-        unsigned lane = threadIdx.x & 31, base = 0;
-        if (lane == 0) base = atomicAdd(&ctl->next_count, unsigned(__popc(m)));
-        base = __shfl_sync(0xffffffffu, base, 0);
+    uint32_t *const next[1] = {&ctl->next_count};
+    const bool take[1] = {alive};
+    uint32_t at[1];
+    block_alloc<1, 256>(next, take, at);
+    {
+        const unsigned m = __ballot_sync(0xffffffffu, alive), lane = threadIdx.x & 31u;
         if (alive) {
-            uint32_t t = base + __popc(m & ((1u << lane) - 1u));
+            const uint32_t t = at[0];
             V3 o = v3(t0.x, t0.y, t0.z), d = v3(t1.x, t1.y, t1.z); float tmin = t0.w;
             Hit h = analytic_closest(sc, o, d, tmin, INFINITY);
             dst.T0[t] = t0;
@@ -1409,7 +1469,9 @@ __global__ void __launch_bounds__(256) k_accum(DScene sc, PathBuf pb, PathBuf ds
             dst.pcg[t] = pb.pcg[s];
             uint32_t key = mesh_cut_hit(sc, o, d, tmin, h.t) ? ray_bin(sc, o, d) : kBins;       // kBins: nothing to traverse
             keys[t] = key;
-            if (key != kBins) atomicAdd(hist + key, 1u);
+            // one atomic per distinct key and warp (skewed keys would serialise per-lane atomics on the hot bins)
+            const unsigned peers = __match_any_sync(m, key);
+            if (key != kBins && lane == unsigned(__ffs(int(peers))) - 1u) atomicAdd(hist + key, unsigned(__popc(peers)));
         }
     }
 }
@@ -1464,12 +1526,23 @@ __global__ void __launch_bounds__(1024) k_iter_end(uint32_t *hist, Ctl *ctl, int
         ctl->shadow_count_closest = 0u; ctl->cursor_closest = 0u;
     }
 }
-// ... and scatter of the slot indices (4 bytes each) to their sorted positions.
+// ... and scatter of the slot indices (4 bytes each) to their sorted positions.  The grid is what is resident at once (or less),
+// a block takes runs of blockDim survivors as k_shadow_prep does, so every lane of a warp makes the same trips.  The lanes of a
+// warp with the same key take consecutive positions with one atomic (the order inside a bin is free: a ray's result does not
+// depend on when or by which lane it is traced).
 __global__ void __launch_bounds__(256) k_bin_scatter(const uint32_t *keys, uint32_t *cursor, const Ctl *ctl, uint32_t *order) {
-    uint32_t t = blockIdx.x*blockDim.x + threadIdx.x;
-    if (t >= ctl->n_surv) return;
-    uint32_t key = keys[t];
-    if (key != kBins) order[atomicAdd(cursor + key, 1u)] = t;     // culled survivors are not visited: no entry needed
+    const uint32_t n = ctl->n_surv, lane = threadIdx.x & 31u;
+    for (uint32_t base = blockIdx.x*blockDim.x; base < n; base += gridDim.x*blockDim.x) {
+        const uint32_t t = base + threadIdx.x;
+        const uint32_t key = t < n ? keys[t] : kBins;
+        const unsigned peers = __match_any_sync(0xffffffffu, key);
+        if (key == kBins) continue;                               // culled survivors are not visited: no entry needed
+        const unsigned leader = unsigned(__ffs(int(peers))) - 1u;
+        uint32_t at = 0;
+        if (lane == leader) at = atomicAdd(cursor + key, unsigned(__popc(peers)));
+        at = __shfl_sync(peers, at, int(leader));
+        order[at + __popc(peers & ((1u << lane) - 1u))] = t;
+    }
 }
 
 // OutputBuffer::addSample (cameras/OutputBuffer.hpp:104-132): running mean in sample order, NaN/Inf samples dropped
