@@ -340,6 +340,15 @@ enum { TGB_BR_ORIGIN = 0, TGB_BR_TMIN = 3, TGB_BR_DIR = 4, TGB_BR_STATUS = 7, TG
        TGB_BR_EMISSION = 12, TGB_BR_FLAGS = 15, TGB_BR_PIXEL = 16, TGB_BR_SEED = 17, TGB_BR_SAMPLE = 18, TGB_BR_DIMENSION = 19,
        TGB_BR_PCG = 20, TGB_BOUNCE_WORDS = 24 };
 int  tgb200_bounce_probe(tgb_ctx *ctx, uint32_t n, const uint32_t *state_in, uint32_t *state_out);
+/* tgb200_bin_probe: the survivor sort of the wavefront loop (the ray-coherence counting sort that orders the next traversal) on n
+ * given keys.  keys[t] is survivor t's key as the survivor hand-off leaves it, in [0, 32767], or 32768 for a survivor that misses
+ * the BVH's top-level cut and is not traversed.  The histogram is counted by the hand-off's own code, then the scan and the
+ * scatter run as in a render, with a render's grid for n survivors.  Out: *n_sorted = the survivors the traversal visits,
+ * order[0 .. *n_sorted) = their indices t in visiting order (bins ascending, any order within a bin; order holds n entries), and
+ * cursors[0 .. 32768) = each bin's end in order.  n must fit the first wavefront (half the context's capacity) and no key may
+ * exceed 32768 (TGB_ERR_INVALID).  keys and order may be NULL when n = 0.  The context's control block and ray counters are left
+ * as they were. */
+int  tgb200_bin_probe(tgb_ctx *ctx, uint32_t n, const uint32_t *keys, uint32_t *order, uint32_t *cursors, uint32_t *n_sorted);
 /* tgb200_shade_variant: the shading kernel the context renders (and tgb200_bounce_probe runs) with, as its template arguments,
  * into variant[0..3]: variant[0] = curves, variant[1] = material sort, variant[2] = lobe set (1: the Lambert-only
  * instantiation), variant[3] = emitter set (1: the Lambert-only instantiation for scenes whose lights are all quads, with no

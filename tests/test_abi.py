@@ -100,6 +100,9 @@ def test_probe_hooks_refuse_a_missing_context():
     st = np.zeros(abi.BOUNCE_WORDS, np.uint32)
     assert L.tgb200_bounce_probe(None, 1, st.ctypes.data, st.ctypes.data) == abi.TGB_ERR_INVALID
     assert L.tgb200_bounce_probe(None, 0, None, None) == abi.TGB_ERR_INVALID
+    cur = np.zeros(abi.BINS, np.uint32); ns = C.c_uint32()
+    assert L.tgb200_bin_probe(None, 1, pix.ctypes.data, pix.ctypes.data, cur.ctypes.data, C.byref(ns)) == abi.TGB_ERR_INVALID
+    assert L.tgb200_bin_probe(None, 0, None, None, None, None) == abi.TGB_ERR_INVALID
     assert L.tgb200_shade_variant(None, pix.ctypes.data) == abi.TGB_ERR_INVALID
 
 

@@ -21,6 +21,8 @@ CURVE_CYLINDER, CURVE_HALF_CYLINDER, CURVE_BCSDF_CYLINDER = 0, 1, 2
 # tgb200_bounce_probe's path-state record: word offsets (uint32 words; float fields are stored as their bits)
 (BR_ORIGIN, BR_TMIN, BR_DIR, BR_STATUS, BR_THROUGHPUT, BR_BOUNCE, BR_EMISSION, BR_FLAGS, BR_PIXEL, BR_SEED, BR_SAMPLE,
  BR_DIMENSION, BR_PCG, BOUNCE_WORDS) = 0, 3, 4, 7, 8, 11, 12, 15, 16, 17, 18, 19, 20, 24
+# bins of the survivor sort (tgb200_bin_probe); the key BINS marks a survivor that is not traversed
+BINS = 1 << 15
 
 f32, u32, i32, u64 = C.c_float, C.c_uint32, C.c_int32, C.c_uint64
 F3, F9 = f32*3, f32*9
@@ -111,6 +113,6 @@ EXPORTS = [
     "tgb200_create", "tgb200_render_tiles", "tgb200_render_resident", "tgb200_clear_framebuffer",
     "tgb200_read_framebuffer", "tgb200_write_framebuffer", "tgb200_generate_work", "tgb200_render_adaptive", "tgb200_framebuffer_device_ptr", "tgb200_trace_closest", "tgb200_shard_tiles", "tgb200_pack_tiles", "tgb200_unpack_tiles",
     "tgb200_get_stats", "tgb200_set_profiling", "tgb200_set_stream", "tgb200_scene_info", "tgb200_reset_stats", "tgb200_bvh_selftest", "tgb200_hair_selftest", "tgb200_qbvh_selftest", "tgb200_shadow_walk_count", "tgb200_bsdf_probe", "tgb200_bsdf_sample_probe", "tgb200_light_probe",
-    "tgb200_choose_light_probe", "tgb200_shadow_probe", "tgb200_bounce_probe", "tgb200_shade_variant", "tgb200_abort", "tgb200_clear_abort", "tgb200_destroy", "tgb200_last_error",
+    "tgb200_choose_light_probe", "tgb200_shadow_probe", "tgb200_bounce_probe", "tgb200_bin_probe", "tgb200_shade_variant", "tgb200_abort", "tgb200_clear_abort", "tgb200_destroy", "tgb200_last_error",
     "tgb200_abi_version",
 ]

@@ -782,6 +782,9 @@ int set_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed
 }
 
 inline unsigned blocks(uint32_t n, unsigned bs) { return n ? (n + bs - 1)/bs : 1; }
+// Grid of a grid-stride loop kernel (k_regen, k_shadow_prep, k_bin_scatter: 256 threads) for at most `bound` items: the blocks
+// they need, at most `resident` (the context's regen_blocks, prep_blocks or scatter_blocks).  Renders and probes alike.
+inline unsigned loop_grid(uint32_t resident, uint32_t bound) { return std::min(blocks(bound, 256), resident); }
 
 // The wavefront loop: the GPU analogue of renderTile over (pixels of the tiles) x (sample range), with path
 // regeneration: whenever paths finish, their slots are refilled with the next camera paths of the step, so every
@@ -809,7 +812,7 @@ uint32_t enqueue_bounce(tgb_ctx *c, Wavefront &w, const PathBuf &pb, const PathB
     if (ev) cudaEventRecord(ev[0], st);
     ks.shade<<<blocks(bound, ks.shade_paths), ks.shade_block, 0, st>>>(sc, pb, w.sr, bi, w.ctl, w.squeue, c->ctr);
     if (ev) cudaEventRecord(ev[1], st);
-    ks.shadow_prep<<<std::min(blocks(2*bound, 256), c->prep_blocks), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+    ks.shadow_prep<<<loop_grid(c->prep_blocks, 2*bound), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
     if (ev) cudaEventRecord(ev[2], st);
     // the any-hit queue and (scenes with mesh lights) the closest-hit queue
     if (has_bvh) ks.shadow_bvh<<<std::min(blocks(2*bound, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
@@ -826,11 +829,11 @@ void enqueue_iteration(tgb_ctx *c, Wavefront &w, cudaStream_t st, const BatchInf
     PathBuf &pb = w.pb[cur], &nxt = w.pb[cur ^ 1];
     const bool prof = c->profiling;
     if (prof) cudaEventRecord(w.ev_k[slot][0], st);
-    k_regen<<<std::min(blocks(bound, 256), c->regen_blocks), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
+    k_regen<<<loop_grid(c->regen_blocks, bound), 256, 0, st>>>(sc, pb, bi, w.ctl, w.order, w.bin_hist); launches++;
     if (prof) cudaEventRecord(w.ev_k[slot][1], st);
     launches += enqueue_bounce(c, w, pb, nxt, st, bi, bound, prof ? &w.ev_k[slot][2] : nullptr);
     k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, has_bvh ? 1 : 0); launches++;
-    if (has_bvh) { k_bin_scatter<<<std::min(blocks(bound, 256), c->scatter_blocks), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order); launches++; }
+    if (has_bvh) { k_bin_scatter<<<loop_grid(c->scatter_blocks, bound), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order); launches++; }
     if (prof) cudaEventRecord(w.ev_k[slot][7], st);
 }
 
@@ -1204,6 +1207,11 @@ int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
             if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bs, k_bin_scatter, 256, 0);
             if (e != cudaSuccess || br <= 0 || bp <= 0 || bs <= 0) { rc = fail(c, TGB_ERR_CUDA, "loop kernels cannot be resident (%s)", cudaGetErrorString(e)); break; }
             c->regen_blocks = uint32_t(sms)*uint32_t(br); c->prep_blocks = uint32_t(sms)*uint32_t(bp); c->scatter_blocks = uint32_t(sms)*uint32_t(bs);
+            // TGB_LOOP_BLOCKS: at most that many blocks in the whole grid (not per SM), so that a test knows each trip's size
+            if (const char *lb = getenv("TGB_LOOP_BLOCKS")) {
+                const int v = atoi(lb);
+                if (v >= 1) for (uint32_t *g : {&c->regen_blocks, &c->prep_blocks, &c->scatter_blocks}) *g = std::min(*g, uint32_t(v));
+            }
         }
     } while (0);
     if (rc) { g_create_error = c->error; tgb200_destroy(c); return rc; }
@@ -1985,7 +1993,7 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
         if (e != cudaSuccess) break;
         k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, w.sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
                                                             w.squeue, w.ctl, m);
-        c->ks.shadow_prep<<<blocks(m, 256), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
+        c->ks.shadow_prep<<<loop_grid(c->prep_blocks, m), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
         k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(w.squeue2, w.squeue_cl, w.ctl, dout + 8*size_t(off));
         if (sc.n_nodes)
             c->ks.shadow_bvh<<<std::min(blocks(m, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
@@ -2035,7 +2043,7 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
         k_probe_bounce_setup<<<blocks(m, 256), 256, 0, st>>>(sc, pb, din + TGB_BOUNCE_WORDS*size_t(off), pix_id, pix_seed, pix_first,
                                                             pix_base, w.bin_keys, w.bin_hist, o, m);
         k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, sc.n_nodes ? 1 : 0);
-        if (sc.n_nodes) k_bin_scatter<<<blocks(m, 256), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
+        if (sc.n_nodes) k_bin_scatter<<<loop_grid(c->scatter_blocks, m), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
         enqueue_bounce(c, w, pb, dst, st, bi, m, nullptr);
         k_probe_bounce_alive<<<blocks(m, 256), 256, 0, st>>>(dst, w.ctl, o);
         k_probe_bounce_finished<<<blocks(m, 256), 256, 0, st>>>(pb, c->R, o, m);
@@ -2045,6 +2053,37 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
     }
     if (e == cudaSuccess) e = b.download(state_out, dout, TGB_BOUNCE_WORDS*size_t(n));
     return b.finish(e, "bounce_probe");
+}
+
+int tgb200_bin_probe(tgb_ctx *c, uint32_t n, const uint32_t *keys, uint32_t *order, uint32_t *cursors, uint32_t *n_sorted) {
+    if (!c || !cursors || !n_sorted || (n && (!keys || !order))) return TGB_ERR_INVALID;
+    Wavefront &w = c->wf[0];
+    if (n > w.capacity) return fail(c, TGB_ERR_INVALID, "%u survivors: wavefront 0 holds %u", n, w.capacity);
+    for (uint32_t i = 0; i < n; ++i)
+        if (keys[i] > kBins) return fail(c, TGB_ERR_INVALID, "survivor %u: key %u is past kBins (%u)", i, keys[i], kBins);
+    CU(cudaSetDevice(c->device));
+    ProbeBufs b(c);
+    uint32_t *dkeys = nullptr;
+    cudaError_t e = b.upload(&dkeys, keys, n);
+    if (e == cudaSuccess) e = b.save_state();
+    const cudaStream_t st = c->stream;
+    // n survivors just handed over by k_accum, with no camera path left to issue (as tgb200_bounce_probe stages them)
+    Ctl init; std::memset(&init, 0, sizeof(Ctl));
+    init.next_count = n; init.capacity = w.capacity;
+    if (e == cudaSuccess) e = cudaMemcpyAsync(w.ctl, &init, sizeof(Ctl), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(w.bin_hist, 0, kBins*sizeof(uint32_t), st);
+    if (e == cudaSuccess) {
+        k_probe_bin_setup<<<blocks(n, 256), 256, 0, st>>>(dkeys, w.bin_keys, w.bin_hist, n);
+        k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, 1);
+        k_bin_scatter<<<loop_grid(c->scatter_blocks, n), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = b.download(n_sorted, &w.ctl->n_sorted, 1);
+    if (e == cudaSuccess) e = b.download(cursors, w.bin_hist, kBins);
+    // (init and n_sorted are host variables the stream reads and writes: wait before reading n_sorted or leaving)
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e == cudaSuccess && *n_sorted) e = b.download(order, w.order, std::min(*n_sorted, n));
+    return b.finish(e, "bin_probe");
 }
 
 int tgb200_shade_variant(const tgb_ctx *c, uint32_t *variant) {

@@ -1,7 +1,7 @@
 // Kernels of the test hooks (tgb200_bsdf_probe, tgb200_bsdf_sample_probe, tgb200_light_probe, tgb200_choose_light_probe,
 // tgb200_shadow_probe): one thread per input, each calling the device functions k_shade calls (bsdf_eval / bsdf_pdf / bsdf_sample
 // with k_shade's template arguments, light_sample_direct + light_hit_direct / mesh_direct_pdf, choose_light, light_query).
-// tgb200_bounce_probe's kernels only set up and read back path state around the renderer's own wavefront kernels.
+// tgb200_bounce_probe's and tgb200_bin_probe's kernels only set up and read back state around the renderer's own wavefront kernels.
 // Nothing here restates their arithmetic.
 #pragma once
 #include "tgb_wavefront.cuh"
@@ -203,6 +203,17 @@ __global__ void __launch_bounds__(256) k_probe_bounce_finished(PathBuf pb, const
     o[TGB_BR_DIMENSION] = __float_as_uint(pb.T1[i].w) & 0xFFFFu;
     const uint64_t pcg = pb.pcg[i];
     o[TGB_BR_PCG] = uint32_t(pcg); o[TGB_BR_PCG + 1] = uint32_t(pcg >> 32);
+}
+
+// tgb200_bin_probe, before k_iter_end: keys[t] of n survivors as k_accum leaves them in bin_keys, counted in the cleared histogram
+// by k_accum's own bin_count (the warp's lanes below n take part, as k_accum's alive lanes do)
+__global__ void __launch_bounds__(256) k_probe_bin_setup(const uint32_t *in, uint32_t *keys, uint32_t *hist, uint32_t n) {
+    const uint32_t t = blockIdx.x*blockDim.x + threadIdx.x;
+    const unsigned m = __ballot_sync(0xffffffffu, t < n);
+    if (t >= n) return;
+    const uint32_t key = in[t];
+    keys[t] = key;
+    bin_count(hist, m, key);
 }
 
 __global__ void __launch_bounds__(128) k_probe_choose_light(DScene sc, uint32_t seed, const uint32_t *pixel_id, uint32_t sample,

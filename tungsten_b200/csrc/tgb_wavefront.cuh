@@ -1409,6 +1409,14 @@ __global__ void __launch_bounds__(kTraceBlock, CURVES ? TGB_MINB_CURVES : TGB_MI
     if ((threadIdx.x & 31) == 0 && blocked) atomicAdd(&ctr->shadow_hits, (unsigned long long)blocked);
 }
 
+// A survivor's ray-coherence key into the histogram of the counting sort, one atomic per distinct key and warp (skewed keys would
+// serialise per-lane atomics on the hot bins).  m: the lanes of the warp that call it, each with its own key; kBins is not counted.
+TGB_D void bin_count(uint32_t *hist, unsigned m, uint32_t key) {
+    const unsigned lane = threadIdx.x & 31u;
+    const unsigned peers = __match_any_sync(m, key);
+    if (key != kBins && lane == unsigned(__ffs(int(peers))) - 1u) atomicAdd(hist + key, unsigned(__popc(peers)));
+}
+
 // Fold this bounce's direct light + surface emission into the path (order as in handleSurface:537-543), apply the
 // NaN guards of traceSample (PathTracer.cpp:119-122,130), store finished samples, and MOVE the survivors' persistent
 // state to the front of the other state buffer (physical compaction: all later accesses are coalesced, no slot
@@ -1456,7 +1464,7 @@ __global__ void __launch_bounds__(256) k_accum(DScene sc, PathBuf pb, PathBuf ds
     uint32_t at[1];
     block_alloc<1, 256>(next, take, at);
     {
-        const unsigned m = __ballot_sync(0xffffffffu, alive), lane = threadIdx.x & 31u;
+        const unsigned m = __ballot_sync(0xffffffffu, alive);
         if (alive) {
             const uint32_t t = at[0];
             V3 o = v3(t0.x, t0.y, t0.z), d = v3(t1.x, t1.y, t1.z); float tmin = t0.w;
@@ -1469,9 +1477,7 @@ __global__ void __launch_bounds__(256) k_accum(DScene sc, PathBuf pb, PathBuf ds
             dst.pcg[t] = pb.pcg[s];
             uint32_t key = mesh_cut_hit(sc, o, d, tmin, h.t) ? ray_bin(sc, o, d) : kBins;       // kBins: nothing to traverse
             keys[t] = key;
-            // one atomic per distinct key and warp (skewed keys would serialise per-lane atomics on the hot bins)
-            const unsigned peers = __match_any_sync(m, key);
-            if (key != kBins && lane == unsigned(__ffs(int(peers))) - 1u) atomicAdd(hist + key, unsigned(__popc(peers)));
+            bin_count(hist, m, key);
         }
     }
 }

@@ -55,6 +55,7 @@ def load():
     L.tgb200_choose_light_probe.argtypes = [vp, u32, u32, vp, u32, vp, vp]
     L.tgb200_shadow_probe.argtypes = [vp, u32, vp, vp, vp]
     L.tgb200_bounce_probe.argtypes = [vp, u32, vp, vp]
+    L.tgb200_bin_probe.argtypes = [vp, u32, vp, vp, vp, C.POINTER(u32)]
     L.tgb200_shade_variant.argtypes = [vp, vp]
     L.tgb200_destroy.argtypes = [vp]; L.tgb200_destroy.restype = None
     L.tgb200_last_error.argtypes = [vp]; L.tgb200_last_error.restype = C.c_char_p
@@ -154,6 +155,17 @@ class Context:
         out = np.zeros_like(states)
         self._check(self.L.tgb200_bounce_probe(self.h, len(states), states.ctypes.data, out.ctypes.data))
         return out
+
+    def bin_probe(self, keys):
+        """tgb200_bin_probe: uint32 keys of n survivors (abi.BINS: not traversed) in, (order[:n_sorted], cursors [abi.BINS],
+        n_sorted) of the survivor sort out."""
+        keys = np.ascontiguousarray(keys, dtype=np.uint32).reshape(-1)
+        order = np.zeros(max(len(keys), 1), np.uint32)
+        cursors = np.zeros(abi.BINS, np.uint32)
+        n_sorted = C.c_uint32()
+        self._check(self.L.tgb200_bin_probe(self.h, len(keys), keys.ctypes.data, order.ctypes.data, cursors.ctypes.data,
+                                            C.byref(n_sorted)))
+        return order[:min(n_sorted.value, len(keys))], cursors, n_sorted.value
 
     def shade_variant(self):
         """The k_shade instantiation the context renders with, as its template arguments: '<CURVES, MATSORT, LS>'."""
