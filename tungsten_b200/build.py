@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libtgb200.so")
 SOURCES = ["tgb200_api.cu", "bvh_build.cpp", "hair_tables.cpp", "sobol_blob.cpp"]
-HEADERS = ["tgb_device.cuh", "tgb_wavefront.cuh", "tgb_probe.cuh", "bvh_build.h", "hair_tables.h", os.path.join("..", "..", "include", "tgb200.h")]
+HEADERS = ["tgb_device.cuh", "tgb_wavefront.cuh", "tgb_probe.cuh", "tgb_scene.cuh", "bvh_build.h", "hair_tables.h", os.path.join("..", "..", "include", "tgb200.h")]
 BLOB = os.path.join(HERE, "data", "sobol_1024x32.u32")
 
 # -fmad=false: the reference is built without FMA contraction (CMakeLists.txt:17-19); radiance parity needs

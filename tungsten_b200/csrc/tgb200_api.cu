@@ -1,7 +1,7 @@
-// C ABI of libtgb200.so (include/tgb200.h): scene preparation, device upload, wavefront render loop.
-// Host logic mirrors the reference's TraceableScene constructor + PathTraceIntegrator (prepare, tile
-// dicing, sample stepping); all rendering arithmetic runs in the CUDA kernels of tgb_wavefront.cuh.
-// There is NO CPU fallback: without a CUDA device every entry point fails with TGB_ERR_NO_DEVICE.
+// C ABI of libtgb200.so (include/tgb200.h): device upload of a prepared scene (tgb_scene.cuh), wavefront render loop.
+// Host logic mirrors the reference's PathTraceIntegrator (tile dicing, sample stepping); all rendering arithmetic runs in the
+// CUDA kernels of tgb_wavefront.cuh.  There is NO CPU fallback: without a CUDA device every entry point fails with
+// TGB_ERR_NO_DEVICE (tgb200_create once the desc has passed its checks).
 #include <algorithm>
 #include <atomic>
 #include <cmath>
@@ -12,12 +12,10 @@
 #include <string>
 #include <vector>
 
-#include "bvh_build.h"
-#include "hair_tables.h"
 #include "tgb_wavefront.cuh"
 #include "tgb_probe.cuh"
+#include "tgb_scene.cuh"
 
-extern "C" const unsigned char tgb_sobol_blob[];      // sobol_blob.cpp (.incbin of data/sobol_1024x32.u32)
 
 using namespace tgb;
 
@@ -38,8 +36,6 @@ struct Group {
 };
 
 namespace {
-
-thread_local std::string g_create_error;
 
 // One wavefront: the loop state of its share of a (sub)step's camera paths.  A context runs two of them, each on its own stream,
 // so that one wavefront's traversal kernels (ALU bound) run alongside the other's streaming kernels (HBM bound).
@@ -64,6 +60,7 @@ struct Kernels {
     decltype(&k_shadow_prep<false>) shadow_prep = nullptr;
     decltype(&k_shadow_bvh<false, false>) shadow_bvh = nullptr;
     decltype(&k_hook_persist<false>) hook_persist = nullptr;
+    uint32_t variant[4] = {};       // what tgb200_shade_variant reports: curves, material-sorted, Lambert-only, quad emitters
 };
 
 }  // namespace
@@ -81,14 +78,10 @@ struct tgb_ctx {
     // wavefront storage
     uint32_t capacity = 0;          // paths in flight, both wavefronts together
     Wavefront wf[2];                // the hooks run on wf[0]'s buffers
-    bool mesh_lights = false;       // a mesh is a light: closest-hit shadow queries exist, k_shadow_bvh<., false> runs
     uint32_t persist_blocks = 0;    // grid of the persistent traversal kernels (per wavefront)
     uint32_t regen_blocks = 0, prep_blocks = 0, scatter_blocks = 0;   // largest grids of the grid-stride kernels (resident blocks)
-    bool diffuse_only = false;      // all surfaces Lambert / null: k_shade<.., .., 1>
-    bool quad_emitters = false;     // ... and only quad lights, constant textures: k_shade<.., .., 1, 1>
-    bool sort_materials = false;    // >= 2 lobe models in use: k_shade deals the paths of a block to its threads by BSDF type
-    bool has_curves = false;        // selects the kernel instantiations with the curve-segment test and per-hit epsilon
-    Kernels ks;                     // the instantiations the five flags above select
+    bool has_curves = false;        // the probes pick their instantiations with the curve-segment test and per-hit epsilon
+    Kernels ks;                     // the instantiations select_kernels chose for the scene
     int n_bsdfs = 0; std::vector<uint32_t> prim_types; std::vector<int> light_ids;   // host copies for the test hooks' argument checks
     float4 *R = nullptr; size_t res_capacity = 0;   // finished radiance per path of the (sub)step
     cudaStream_t own_stream = nullptr;
@@ -138,548 +131,108 @@ int dev_upload(tgb_ctx *c, const T **out, const std::vector<T> &v) {
     return TGB_OK;
 }
 
-V3 f3(const float *p) { return v3(p[0], p[1], p[2]); }
-void transpose3(const float *m, float *t) {
-    t[0] = m[0]; t[1] = m[3]; t[2] = m[6]; t[3] = m[1]; t[4] = m[4]; t[5] = m[7]; t[6] = m[2]; t[7] = m[5]; t[8] = m[8];
-}
-
-// ---- host-side "prepareForRender" pieces (fp32, reference operation order; compiled with -fmad=false) ----
-float filter_width(uint32_t f) {
-    switch (f) { case TGB_FILTER_DIRAC: return 0.0f; case TGB_FILTER_BOX: return 0.5f; case TGB_FILTER_TENT: return 1.0f; default: return 2.0f; }
-}
-float filter_eval(uint32_t f, float x) {                        // cameras/ReconstructionFilter.hpp:171-193
-    switch (f) {
-    case TGB_FILTER_BOX: return (x >= -0.5f && x <= 0.5f) ? 1.0f : 0.0f;
-    case TGB_FILTER_TENT: return 1.0f - std::fabs(x);
-    case TGB_FILTER_GAUSSIAN: { const float Alpha = 2.0f; return std::max(std::exp(-Alpha*x*x) - std::exp(-Alpha*4.0f), 0.0f); }
-    case TGB_FILTER_MITCHELL: { x = std::fabs(x); const float B = 1.0f/3.0f, C = 1.0f/3.0f;
-        if (x < 1.0f) return 1.0f/6.0f*((12.0f - 9.0f*B - 6.0f*C)*x*x*x + (-18.0f + 12.0f*B + 6.0f*C)*x*x + (6.0f - 2.0f*B));
-        else if (x < 2.0f) return 1.0f/6.0f*((-B - 6.0f*C)*x*x*x + (6.0f*B + 30.0f*C)*x*x + (-12.0f*B - 48.0f*C)*x + (8.0f*B + 24.0f*C));
-        return 0.0f; }
-    case TGB_FILTER_CATMULL_ROM: { x = std::fabs(x);
-        if (x < 1.0f) return 1.0f/6.0f*((12.0f - 3.0f)*x*x*x + (-18.0f + 3.0f)*x*x + 6.0f);
-        else if (x < 2.0f) return 1.0f/6.0f*(-3.0f*x*x*x + 15.0f*x*x - 24.0f*x + 12.0f);
-        return 0.0f; }
-    case TGB_FILTER_LANCZOS: { x = std::fabs(x);
-        if (x == 0.0f) return 1.0f;
-        else if (x < 2.0f) return std::sin(PI_F*x)*std::sin(PI_F*x/2.0f)/(PI_F*PI_F*x*x/2.0f);
-        return 0.0f; }
-    default: return 0.0f;
-    }
-}
-void filter_precompute(DCamera &cam) {                          // cameras/ReconstructionFilter.cpp:34-58
-    const int R = 31;
-    float width = filter_width(cam.filter);
-    cam.filter_bin = width/R;
-    std::memset(cam.filter_cdf, 0, sizeof(cam.filter_cdf));
-    if (cam.filter == TGB_FILTER_BOX || cam.filter == TGB_FILTER_DIRAC) return;
-    float f[32], sum = 0.0f;
-    for (int i = 0; i < R; ++i) { f[i] = filter_eval(cam.filter, (i*width)/R); sum += f[i]; }
-    cam.filter_cdf[0] = 0.0f;
-    for (int i = 1; i < R; ++i) cam.filter_cdf[i] = cam.filter_cdf[i - 1] + f[i - 1]/sum;
-    cam.filter_cdf[R] = 1.0f;
-}
-float h_dielectric_reflectance(float eta, float cosThetaI) {    // bsdfs/Fresnel.hpp:75-92
-    if (cosThetaI < 0.0f) { eta = 1.0f/eta; cosThetaI = -cosThetaI; }
-    float sinThetaTSq = eta*eta*(1.0f - cosThetaI*cosThetaI);
-    if (sinThetaTSq > 1.0f) return 1.0f;
-    float cosThetaT = std::sqrt(std::max(1.0f - sinThetaTSq, 0.0f));
-    float Rs = (eta*cosThetaI - cosThetaT)/(eta*cosThetaI + cosThetaT);
-    float Rp = (eta*cosThetaT - cosThetaI)/(eta*cosThetaT + cosThetaI);
-    return (Rs*Rs + Rp*Rp)*0.5f;
-}
-float diffuse_fresnel(float ior, int sampleCount) {             // bsdfs/Fresnel.hpp:141-153
-    double acc = 0.0;
-    float fb = h_dielectric_reflectance(ior, 0.0f);
-    for (int i = 1; i <= sampleCount; ++i) {
-        float cosThetaSq = float(i)/sampleCount;
-        float fa = h_dielectric_reflectance(ior, std::min(std::sqrt(cosThetaSq), 1.0f));
-        acc += double(fa + fb)*(0.5/sampleCount);
-        fb = fa;
-    }
-    return float(acc);
-}
-uint32_t bsdf_lobes(const tgb_bsdf &b) {
-    switch (b.type) {
-    case TGB_BSDF_NULL: return 0;
-    case TGB_BSDF_LAMBERT: return LOBE_DIFFUSE_R;
-    case TGB_BSDF_ROUGH_CONDUCTOR: return LOBE_GLOSSY_R;
-    case TGB_BSDF_ROUGH_DIELECTRIC: return b.enable_refraction ? (LOBE_GLOSSY_R | LOBE_GLOSSY_T) : LOBE_GLOSSY_R;
-    case TGB_BSDF_PLASTIC: return LOBE_SPEC_R | LOBE_DIFFUSE_R;
-    case TGB_BSDF_ROUGH_PLASTIC: return LOBE_GLOSSY_R | LOBE_DIFFUSE_R;
-    case TGB_BSDF_MIRROR: case TGB_BSDF_CONDUCTOR: return LOBE_SPEC_R;                   // MirrorBsdf.cpp:13, ConductorBsdf.cpp:19
-    case TGB_BSDF_DIELECTRIC: return b.enable_refraction ? (LOBE_SPEC_R | LOBE_SPEC_T) : LOBE_SPEC_R;   // DielectricBsdf.cpp:174-180
-    case TGB_BSDF_SMOOTH_COAT: return LOBE_SPEC_R;          // | substrate lobes, added by upload_scene
-    case TGB_BSDF_ROUGH_COAT: return LOBE_GLOSSY_R;         // | substrate lobes (RoughCoatBsdf.cpp:301-306)
-    case TGB_BSDF_HAIR: return LOBE_GLOSSY_R | LOBE_GLOSSY_T | LOBE_ANISO;                  // bsdfs/HairBcsdf.cpp:20
-    default: return 0xFFFFFFFFu;
-    }
-}
-
-struct HostTex { DTex d; V3 maxv; std::vector<float> marg_pdf, marg_cdf, pdf, cdf; bool has_dist = false; };
-
-// BitmapTexture::makeSamplable(MAP_SPHERICAL) + Distribution2D (textures/BitmapTexture.cpp:400-431,
-// sampling/Distribution2D.hpp:18-46)
-void build_spherical_distribution(const tgb_texture &t, HostTex &ht) {
-    int w = int(t.res_u), h = int(t.res_v); bool clampm = (t.flags >> 1) & 1;
-    std::vector<float> weights(size_t(w)*h);
-    for (int y = 0, idx = 0; y < h; ++y) {
-        float rowWeight = 1.0f;
-        rowWeight *= std::sin((y*PI_F)/h);
-        for (int x = 0; x < w; ++x, ++idx) {
-            const float *p = t.texels + 3*size_t(idx);
-            weights[idx] = max_comp(v3(p[0], p[1], p[2]))*rowWeight;
-        }
-    }
-    // in-place max dilation, x then y, wrapping unless the texture clamps (BitmapTexture.cpp:411-428)
-    for (int y = 0; y < h; ++y) {
-        for (int x = 0; x < w - 1; ++x) weights[x + y*w] = std::max(weights[x + y*w], weights[x + 1 + y*w]);
-        if (!clampm) weights[y*w] = weights[w - 1 + y*w] = std::max(weights[w - 1 + y*w], weights[y*w]);
-        for (int x = w - 1; x > 0; --x) weights[x + y*w] = std::max(weights[x + y*w], weights[x - 1 + y*w]);
-    }
-    for (int x = 0; x < w; ++x) {
-        for (int y = 0; y < h - 1; ++y) weights[x + y*w] = std::max(weights[x + y*w], weights[x + (y + 1)*w]);
-        if (!clampm) weights[x] = weights[x + (h - 1)*w] = std::max(weights[x], weights[x + (h - 1)*w]);
-        for (int y = h - 1; y > 0; --y) weights[x + y*w] = std::max(weights[x + y*w], weights[x + (y - 1)*w]);
-    }
-    // Distribution2D (sampling/Distribution2D.hpp:18-60)
-    ht.pdf = weights; ht.cdf.assign(size_t(w + 1)*h, 0.0f); ht.marg_pdf.assign(h, 0.0f); ht.marg_cdf.assign(h + 1, 0.0f);
-    for (int y = 0; y < h; ++y) {
-        int idxP = y*w, idxC = y*(w + 1);
-        ht.cdf[idxC] = 0.0f;
-        for (int x = 0; x < w; ++x, ++idxP, ++idxC) { ht.marg_pdf[y] += ht.pdf[idxP]; ht.cdf[idxC + 1] = ht.cdf[idxC] + ht.pdf[idxP]; }
-        ht.marg_cdf[y + 1] = ht.marg_cdf[y] + ht.marg_pdf[y];
-    }
-    for (int y = 0; y < h; ++y) {
-        int idxP = y*w, idxC = y*(w + 1), idxTail = idxC + w;
-        float rowWeight = ht.cdf[idxTail];
-        if (rowWeight < 1e-4f) { for (int x = 0; x < w; ++x, ++idxP, ++idxC) { ht.pdf[idxP] = 1.0f/w; ht.cdf[idxC] = x/float(w); } }
-        else { for (int x = 0; x < w; ++x, ++idxP, ++idxC) { ht.pdf[idxP] /= rowWeight; ht.cdf[idxC] /= rowWeight; } }
-        ht.cdf[idxTail] = 1.0f;
-    }
-    float totalWeight = ht.marg_cdf[h];
-    for (float &p : ht.marg_pdf) p /= totalWeight;
-    for (float &cc : ht.marg_cdf) cc /= totalWeight;
-    ht.marg_cdf[h] = 1.0f;
-    ht.has_dist = true;
-}
-
-// The BVH build switches: BvhOptions' defaults, overridden from the environment (DESIGN.md section 6).  tgb200_create and the
-// host-only BVH checks read them alike, so the checks walk the tree tgb200_create builds.
-BvhOptions bvh_options() {
-    BvhOptions o;
-    if (const char *e = getenv("TGB_TRI_LEAF")) o.tri_leaf = uint32_t(atoi(e));
-    if (const char *e = getenv("TGB_TRI_COST")) o.tri_cost = float(atof(e));
-    if (const char *e = getenv("TGB_CURVE_LEAF")) o.curve_leaf = uint32_t(atoi(e));
-    if (const char *e = getenv("TGB_CURVE_COST")) o.curve_cost = float(atof(e));
-    if (const char *e = getenv("TGB_CUT_BOXES")) o.max_cut = size_t(std::min(16, std::max(4, atoi(e))));
-    return o;
-}
-
-// World bounds of a quad's four corners or a cube's eight
-Aabb analytic_bounds(const DPrim &p) {
-    Aabb b = {{INFINITY, INFINITY, INFINITY}, {-INFINITY, -INFINITY, -INFINITY}};
-    auto grow = [&](V3 q) { float v[3] = {q.x, q.y, q.z}; for (int a = 0; a < 3; ++a) { b.lo[a] = std::min(b.lo[a], v[a]); b.hi[a] = std::max(b.hi[a], v[a]); } };
-    if (p.type == TGB_PRIM_QUAD) { grow(p.base); grow(p.base + p.edge0); grow(p.base + p.edge1); grow(p.base + p.edge0 + p.edge1); }
-    else for (int j = 0; j < 8; ++j) grow(p.pos + m3mul(p.rot, v3((j & 1 ? p.scale.x : -p.scale.x), (j & 2 ? p.scale.y : -p.scale.y), (j & 4 ? p.scale.z : -p.scale.z))));
-    return b;
-}
-
-int upload_scene(tgb_ctx *c, const tgb_scene_desc *d) {
-    const tgb_camera &cam = d->camera;
-    DScene &sc = c->sc;
-    sc.set = d->settings;
-    // camera precompute (cameras/PinholeCamera.cpp:28-35, Camera.cpp:37-42)
-    sc.cam.pos = f3(cam.pos); std::memcpy(sc.cam.m, cam.xform, sizeof(sc.cam.m));
-    float fovRad = cam.fov_deg*(PI_F/180.0f);
-    sc.cam.plane_dist = 1.0f/std::tan(fovRad*0.5f);
-    sc.cam.ratio = cam.res_y/float(cam.res_x);
-    sc.cam.pixel_size_x = 1.0f/cam.res_x;
-    sc.cam.res_x = cam.res_x; sc.cam.res_y = cam.res_y; sc.cam.filter = cam.filter;
-    filter_precompute(sc.cam);
-    c->res_x = cam.res_x; c->res_y = cam.res_y;
-
-    // ---- textures
-    std::vector<HostTex> tex(d->n_textures + 1);
-    for (uint32_t i = 0; i < d->n_textures; ++i) {
-        const tgb_texture &t = d->textures[i]; DTex &o = tex[i].d;
-        std::memset(&o, 0, sizeof(o));
-        o.type = t.type; o.value = f3(t.value); o.value2 = f3(t.value2); o.res_u = int(t.res_u); o.res_v = int(t.res_v); o.flags = t.flags;
-        if (t.type == TGB_TEX_BITMAP) {
-            if (!t.texels || !t.res_u || !t.res_v) return fail(c, TGB_ERR_INVALID, "bitmap texture %u has no texels", i);
-            size_t n = size_t(t.res_u)*t.res_v;
-            V3 acc = v3s(0.0f), mx = v3s(0.0f);
-            for (size_t k = 0; k < n; ++k) { V3 cc = f3(t.texels + 3*k); acc = acc + cc/float(n); mx = v3(std::max(mx.x, cc.x), std::max(mx.y, cc.y), std::max(mx.z, cc.z)); }
-            o.avg = acc; tex[i].maxv = mx;
-            std::vector<float> tx(t.texels, t.texels + 3*n);
-            int rc = dev_upload(c, &o.texels, tx); if (rc) return rc;
-        } else if (t.type == TGB_TEX_CHECKER) {
-            o.avg = (o.value + o.value2)*0.5f;
-            tex[i].maxv = v3(std::max(o.value.x, o.value2.x), std::max(o.value.y, o.value2.y), std::max(o.value.z, o.value2.z));
-        } else if (t.type == TGB_TEX_CONSTANT) { o.avg = o.value; tex[i].maxv = o.value; }
-        else return fail(c, TGB_ERR_UNSUPPORTED, "texture type %u is outside the hot path", t.type);
-    }
-    { DTex &o = tex[d->n_textures].d; std::memset(&o, 0, sizeof(o)); o.type = TGB_TEX_CONSTANT; o.value = v3s(1.0f); o.avg = o.value; tex[d->n_textures].maxv = o.value; }
-
-    // ---- bsdfs
-    std::vector<DBsdf> bsdfs(d->n_bsdfs);
-    for (uint32_t i = 0; i < d->n_bsdfs; ++i) {
-        const tgb_bsdf &b = d->bsdfs[i]; DBsdf &o = bsdfs[i];
-        std::memset(&o, 0, sizeof(o));
-        o.type = b.type; o.lobes = bsdf_lobes(b);
-        if (o.lobes == 0xFFFFFFFFu) return fail(c, TGB_ERR_UNSUPPORTED, "bsdf type %u is outside the hot path", b.type);
-        if (b.albedo_tex < 0 || uint32_t(b.albedo_tex) >= d->n_textures) return fail(c, TGB_ERR_INVALID, "bsdf %u: bad albedo texture", i);
-        bool rough = b.type == TGB_BSDF_ROUGH_CONDUCTOR || b.type == TGB_BSDF_ROUGH_DIELECTRIC || b.type == TGB_BSDF_ROUGH_PLASTIC || b.type == TGB_BSDF_ROUGH_COAT;
-        if (rough && (b.roughness_tex < 0 || uint32_t(b.roughness_tex) >= d->n_textures)) return fail(c, TGB_ERR_INVALID, "bsdf %u: bad roughness texture", i);
-        o.dist = b.distribution; o.albedo_tex = b.albedo_tex; o.rough_tex = b.roughness_tex;
-        o.ior = b.ior; o.inv_ior = 1.0f/b.ior; o.eta = f3(b.eta); o.k = f3(b.k); o.enable_t = b.enable_refraction; o.substrate = b.substrate;
-        if (b.type == TGB_BSDF_SMOOTH_COAT || b.type == TGB_BSDF_ROUGH_COAT) {             // SmoothCoatBsdf.cpp:218-223, RoughCoatBsdf.cpp:301-306
-            if (b.substrate < 0 || uint32_t(b.substrate) >= d->n_bsdfs || d->bsdfs[b.substrate].type == TGB_BSDF_SMOOTH_COAT ||
-                d->bsdfs[b.substrate].type == TGB_BSDF_ROUGH_COAT || d->bsdfs[b.substrate].type == TGB_BSDF_HAIR)
-                return fail(c, TGB_ERR_UNSUPPORTED, "bsdf %u: a coat needs a substrate that is neither a coat nor the hair BCSDF", i);
-            o.scaled_sigma_a = f3(b.sigma_a)*b.thickness;
-            o.avg_transmittance = std::exp(-2.0f*avg(o.scaled_sigma_a));
-            o.lobes = (b.type == TGB_BSDF_SMOOTH_COAT ? LOBE_SPEC_R : LOBE_GLOSSY_R) | bsdf_lobes(d->bsdfs[b.substrate]);
-        }
-        if (b.type == TGB_BSDF_HAIR) {                                                    // bsdfs/HairBcsdf.cpp:422-446
-            HairTables ht;
-            hair_precompute(b.hair_roughness, b.hair_scale_angle_deg, b.sigma_a, ht);
-            for (int p = 0; p < 3; ++p) {
-                o.hair_v[p] = ht.v[p];
-                int rc = dev_upload(c, &o.hair_table[p], ht.lobe[p].table); if (rc) return rc;
-                rc = dev_upload(c, &o.hair_pdfs[p], ht.lobe[p].pdfs); if (rc) return rc;
-                rc = dev_upload(c, &o.hair_cdfs[p], ht.lobe[p].cdfs); if (rc) return rc;
-                rc = dev_upload(c, &o.hair_sums[p], ht.lobe[p].sums); if (rc) return rc;
-            }
-            o.hair_scale_rad = ht.scale_angle_rad;
-        }
-        if (b.type == TGB_BSDF_PLASTIC || b.type == TGB_BSDF_ROUGH_PLASTIC) {             // bsdfs/PlasticBsdf.cpp:179-185
-            o.scaled_sigma_a = f3(b.sigma_a)*b.thickness;
-            o.avg_transmittance = std::exp(-2.0f*avg(o.scaled_sigma_a));
-            o.diffuse_fresnel = diffuse_fresnel(b.ior, 1000000);
-            o.substrate_weight = avg(tex[b.albedo_tex].d.avg);                             // RoughPlasticBsdf.cpp:215-222
-        }
-    }
-
-    // ---- primitives, lights, triangles
-    std::vector<DPrim> prims(d->n_primitives);
-    std::vector<int> lights, inf_lights, analytic;
-    std::vector<BuildTri> btris; std::vector<uint32_t> tri_prim; std::vector<float4> tri_shade;
-    std::vector<BuildBox> cboxes; std::vector<IsectRecord> crecs; std::vector<uint32_t> cseg_prim;   // curve BVH primitives (kCurvePieces per segment) of all primitives
-    int lightCount = 0;
-    for (uint32_t i = 0; i < d->n_primitives; ++i) {
-        const tgb_primitive &p = d->primitives[i]; DPrim &o = prims[i];
-        std::memset(&o, 0, sizeof(o));
-        o.type = p.type; o.emission_tex = p.emission_tex; o.bsdf_first = p.bsdf_first; o.bsdf_count = p.bsdf_count;
-        if (p.emission_tex >= int(d->n_textures)) return fail(c, TGB_ERR_INVALID, "primitive %u: bad emission texture", i);
-        bool emissive = p.emission_tex >= 0 && max_comp(tex[p.emission_tex].maxv) > 0.0f;  // primitives/Primitive.hpp:111-115
-        bool samplable = true, infinite = false;
-        if (p.type != TGB_PRIM_INFINITE_SPHERE && p.type != TGB_PRIM_INFINITE_SPHERE_CAP && p.type != TGB_PRIM_SKYDOME) {
-            if (p.bsdf_count == 0 || p.bsdf_first + p.bsdf_count > d->n_bsdf_slots) return fail(c, TGB_ERR_INVALID, "primitive %u: bad bsdf range", i);
-            for (uint32_t k = 0; k < p.bsdf_count; ++k) if (d->bsdf_slots[p.bsdf_first + k] >= d->n_bsdfs) return fail(c, TGB_ERR_INVALID, "primitive %u: bad bsdf index", i);
-            // the hair BCSDF is evaluated in the curve's tangent space (Curves::tangentSpace): on any other primitive the kernels
-            // compiled for curve-free scenes would not know the lobe at all
-            if (p.type != TGB_PRIM_CURVES)
-                for (uint32_t k = 0; k < p.bsdf_count; ++k) {
-                    const tgb_bsdf *b = &d->bsdfs[d->bsdf_slots[p.bsdf_first + k]];
-                    for (int hop = 0; hop < 4 && b; ++hop) {
-                        if (b->type == TGB_BSDF_HAIR) return fail(c, TGB_ERR_UNSUPPORTED, "primitive %u: the hair BCSDF on a primitive that is not `curves` is outside the hot path", i);
-                        b = ((b->type == TGB_BSDF_SMOOTH_COAT || b->type == TGB_BSDF_ROUGH_COAT) && b->substrate >= 0 && uint32_t(b->substrate) < d->n_bsdfs) ? &d->bsdfs[b->substrate] : nullptr;
-                    }
-                }
-        }
-        switch (p.type) {
-        case TGB_PRIM_MESH: {
-            if (p.n_tris && (!p.verts || !p.tris)) return fail(c, TGB_ERR_INVALID, "mesh %u has null buffers", i);
-            o.tri_first = uint32_t(btris.size()); o.n_tris = p.n_tris;
-            if (p.smooth) o.flags |= PF_SMOOTH;
-            std::vector<float> areas(p.n_tris), lverts;
-            float total = 0.0f;
-            for (uint32_t k = 0; k < p.n_tris; ++k) {
-                const tgb_triangle &t = p.tris[k];
-                if (t.v0 >= p.n_verts || t.v1 >= p.n_verts || t.v2 >= p.n_verts) return fail(c, TGB_ERR_INVALID, "mesh %u: vertex index out of range", i);
-                const tgb_vertex &a = p.verts[t.v0], &b = p.verts[t.v1], &cc = p.verts[t.v2];
-                BuildTri bt; std::memcpy(bt.v0, a.pos, 12); std::memcpy(bt.v1, b.pos, 12); std::memcpy(bt.v2, cc.pos, 12);
-                btris.push_back(bt); tri_prim.push_back(i);
-                int mat = std::min(std::max(t.material, 0), int(p.bsdf_count) - 1);      // TriangleMesh.cpp:539
-                float4 s0 = make_float4(a.normal[0], a.normal[1], a.normal[2], b.normal[0]);
-                float4 s1 = make_float4(b.normal[1], b.normal[2], cc.normal[0], cc.normal[1]);
-                float4 s2 = make_float4(cc.normal[2], a.uv[0], a.uv[1], b.uv[0]);
-                float4 s3 = make_float4(b.uv[1], cc.uv[0], cc.uv[1], 0.0f);
-                if (mat > 1023 || i >= (1u << 22)) return fail(c, TGB_ERR_UNSUPPORTED, "mesh %u: more than 1024 materials in one mesh or more than 4 Mi primitives", i);
-                uint32_t packed = uint32_t(mat) | (i << 10);            // material | primitive << 10 (make_surface)
-                std::memcpy(&s3.w, &packed, 4);
-                tri_shade.push_back(s0); tri_shade.push_back(s1); tri_shade.push_back(s2); tri_shade.push_back(s3);
-                V3 p0 = f3(a.pos), p1 = f3(b.pos), p2 = f3(cc.pos);
-                areas[k] = length(cross(p1 - p0, p2 - p0))*0.5f;                           // MathUtil::triangleArea
-                total += areas[k];                                                         // TriangleMesh.cpp:556-562
-                if (emissive) { const float *pp[3] = {a.pos, b.pos, cc.pos}; for (int q = 0; q < 3; ++q) for (int r = 0; r < 3; ++r) lverts.push_back(pp[q][r]); }
-            }
-            o.total_area = total;
-            if (p.n_tris == 0 || p.n_verts == 0) emissive = false;                         // isDirac(): not traced, not a light
-            if (emissive) {
-                // Distribution1D over triangle areas (TriangleMesh.cpp:389-403; sampling/Distribution1D.hpp:16-35)
-                std::vector<float> pdf = areas, cdf(p.n_tris + 1);
-                cdf[0] = 0.0f;
-                for (uint32_t k = 0; k < p.n_tris; ++k) cdf[k + 1] = cdf[k] + pdf[k];
-                float tw = cdf[p.n_tris];
-                for (float &x : pdf) x /= tw;
-                for (float &x : cdf) x /= tw;
-                cdf[p.n_tris] = 1.0f;
-                int rc = dev_upload(c, &o.tri_pdf, pdf); if (rc) return rc;
-                rc = dev_upload(c, &o.tri_cdf, cdf); if (rc) return rc;
-                rc = dev_upload(c, &o.light_verts, lverts); if (rc) return rc;
-            }
-            break; }
-        case TGB_PRIM_QUAD: {                                                             // primitives/Quad.cpp:298-316
-            o.base = f3(p.base); o.edge0 = f3(p.edge0); o.edge1 = f3(p.edge1);
-            V3 n = cross(o.edge1, o.edge0);
-            o.area = length(n);
-            o.normal = n/o.area;
-            o.inv_uv_sq0 = 1.0f/length_sq(o.edge0); o.inv_uv_sq1 = 1.0f/length_sq(o.edge1);
-            analytic.push_back(int(i));
-            break; }
-        case TGB_PRIM_CUBE: {                                                             // primitives/Cube.cpp:351-367
-            o.pos = f3(p.pos); o.scale = f3(p.scale);
-            std::memcpy(o.rot, p.rot, sizeof(o.rot)); transpose3(o.rot, o.inv_rot);
-            if (emissive) return fail(c, TGB_ERR_UNSUPPORTED, "emissive cubes are outside the hot path");
-            analytic.push_back(int(i));
-            break; }
-        case TGB_PRIM_INFINITE_SPHERE_CAP: {                                              // primitives/InfiniteSphereCap.cpp:231-247
-            o.normal = f3(p.cap_dir); o.area = p.cap_cos;
-            if (!(p.cap_cos < 1.0f)) return fail(c, TGB_ERR_INVALID, "infinite_sphere_cap %u: cap angle must be positive", i);
-            samplable = p.do_sample != 0; infinite = true;
-            break; }
-        case TGB_PRIM_SKYDOME:                                                            // primitives/Skydome.cpp: an environment sphere with its own prepared image
-            if (p.emission_tex < 0 || tex[p.emission_tex].d.type != TGB_TEX_BITMAP) return fail(c, TGB_ERR_INVALID, "skydome %u: pass the prepared sky image (Skydome::prepareForRender) as a bitmap emission texture", i);
-            o.type = TGB_PRIM_INFINITE_SPHERE; o.flags |= PF_SKYDOME;
-            /* fall through: lookup without rotation (Skydome::directionToUV, Skydome.cpp:29-38) = identity matrices from the caller */
-        case TGB_PRIM_INFINITE_SPHERE: {                                                  // primitives/InfiniteSphere.cpp prepareForRender
-            std::memcpy(o.rot, p.rot, sizeof(o.rot)); transpose3(o.rot, o.inv_rot);
-            if (p.type == TGB_PRIM_SKYDOME) { const float id[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}; std::memcpy(o.rot, id, sizeof(id)); std::memcpy(o.inv_rot, id, sizeof(id)); }
-            samplable = p.do_sample != 0; infinite = true;
-            if (emissive && tex[p.emission_tex].d.type == TGB_TEX_CHECKER) return fail(c, TGB_ERR_UNSUPPORTED, "checker environment maps are outside the hot path");
-            break; }
-        case TGB_PRIM_CURVES: {                                                           // primitives/Curves.cpp:572-613 (nodes arrive prepared)
-            if (p.curve_mode > TGB_CURVE_BCSDF_CYLINDER) return fail(c, TGB_ERR_UNSUPPORTED, "curves %u: mode outside the hot path", i);
-            if (emissive) return fail(c, TGB_ERR_UNSUPPORTED, "emissive curves are outside the hot path");
-            if (p.n_curve_segments && (!p.curve_nodes || !p.curve_segments)) return fail(c, TGB_ERR_INVALID, "curves %u has null buffers", i);
-            if (tex[d->bsdfs[d->bsdf_slots[p.bsdf_first]].albedo_tex].d.type != TGB_TEX_CONSTANT)
-                return fail(c, TGB_ERR_UNSUPPORTED, "curves %u: textured materials on curves are outside the hot path", i);
-            o.curve_mode = p.curve_mode; o.tri_first = uint32_t(cboxes.size()); o.n_tris = p.n_curve_segments*kCurvePieces;   // rebased below
-            for (uint32_t k = 0; k < p.n_curve_segments; ++k) {
-                uint32_t t = p.curve_segments[k];
-                if (t < 2 || t >= p.n_curve_nodes) return fail(c, TGB_ERR_INVALID, "curves %u: segment index out of range", i);
-                const float *n0 = p.curve_nodes + 4*size_t(t - 2), *n1 = n0 + 4, *n2 = n0 + 8;
-                // One BVH primitive per quarter of the segment's parameter range (the reference bounds the whole segment,
-                // curveBox, Curves.cpp:231-243): bounds of the quadratic on [ta, tb] = its end values + the interior extremum,
-                // grown by the largest node width (the width spline is a convex combination of the node widths).
-                float maxW = std::max(std::max(n0[3], n1[3]), n2[3]);
-                for (int piece = 0; piece < kCurvePieces; ++piece) {
-                    BuildBox bb;
-                    float ta = float(piece)/kCurvePieces, tb = float(piece + 1)/kCurvePieces;
-                    for (int a = 0; a < 3; ++a) {
-                        float qa = 0.5f*n0[a] - n1[a] + 0.5f*n2[a], qb = n1[a] - n0[a], qc = 0.5f*(n0[a] + n1[a]);
-                        float fa = (qa*ta + qb)*ta + qc, fb = (qa*tb + qb)*tb + qc;
-                        float lo = std::min(fa, fb), hi = std::max(fa, fb);
-                        float tFlat = -qb/(2.0f*qa);
-                        if (tFlat > ta && tFlat < tb) { float f = (qa*tFlat + qb)*tFlat + qc; lo = std::min(lo, f); hi = std::max(hi, f); }
-                        float slack = 4e-7f*std::max(std::fabs(lo), std::fabs(hi));            // Horner vs the kernel's expanded form
-                        bb.lo[a] = lo - maxW - slack; bb.hi[a] = hi + maxW + slack;
-                        bb.centroid[a] = 0.5f*(lo + hi);
-                    }
-                    cboxes.push_back(bb); cseg_prim.push_back(i);
-                    IsectRecord rec; std::memcpy(rec.f, n0, sizeof(rec.f));        // n0, n1, n2
-                    crecs.push_back(rec);
-                }
-            }
-            break; }
-        default: return fail(c, TGB_ERR_UNSUPPORTED, "primitive type %u is outside the hot path", p.type);
-        }
-        if (emissive) {                                                                   // renderer/TraceableScene.hpp:89-96
-            o.flags |= PF_EMISSIVE; lightCount++;
-            if (samplable) lights.push_back(int(i));
-            if (infinite) inf_lights.push_back(int(i));
-        }
-        if (samplable) o.flags |= PF_SAMPLABLE;
-        if (infinite) o.flags |= PF_INFINITE;
-    }
-    if (lightCount == 0) {                                                                // renderer/TraceableScene.hpp:97-102
-        DPrim o; std::memset(&o, 0, sizeof(o));
-        o.type = TGB_PRIM_INFINITE_SPHERE; o.emission_tex = int(d->n_textures);
-        o.flags = PF_EMISSIVE | PF_SAMPLABLE | PF_INFINITE;
-        const float id[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-        std::memcpy(o.rot, id, sizeof(id)); std::memcpy(o.inv_rot, id, sizeof(id));
-        lights.push_back(int(prims.size())); inf_lights.push_back(int(prims.size()));
-        prims.push_back(o);
-    }
-    for (int li : lights) {
-        DPrim &l = prims[li];
-        if (l.type == TGB_PRIM_INFINITE_SPHERE_CAP && tex[l.emission_tex].d.type == TGB_TEX_BITMAP)
-            return fail(c, TGB_ERR_UNSUPPORTED, "bitmap emission on an infinite_sphere_cap is outside the hot path");
-        if (l.type == TGB_PRIM_INFINITE_SPHERE && tex[l.emission_tex].d.type == TGB_TEX_BITMAP && !tex[l.emission_tex].has_dist)
-            build_spherical_distribution(d->textures[l.emission_tex], tex[l.emission_tex]);
-    }
-    std::vector<DTex> dtex(tex.size());
-    for (size_t i = 0; i < tex.size(); ++i) {
-        if (tex[i].has_dist) {
-            int rc = dev_upload(c, &tex[i].d.marg_pdf, tex[i].marg_pdf); if (rc) return rc;
-            rc = dev_upload(c, &tex[i].d.marg_cdf, tex[i].marg_cdf); if (rc) return rc;
-            rc = dev_upload(c, &tex[i].d.pdf, tex[i].pdf); if (rc) return rc;
-            rc = dev_upload(c, &tex[i].d.cdf, tex[i].cdf); if (rc) return rc;
-        }
-        dtex[i] = tex[i].d;
-    }
-
-    // ---- BVH over every mesh triangle, curve piece and -- only when they are many -- analytic primitive.
-    // Analytic quads/cubes are few in most scenes and are then tested coherently by the kernel that creates a ray; from
-    // TGB_ANALYTIC_BVH_MIN (24) primitives on they get a third SAH tree instead (the reference keeps them in Embree's top-level
-    // user-geometry BVH, renderer/TraceableScene.hpp:112-134), so a ray's cost no longer grows with their number.
-    size_t analytic_bvh_min = 24;
-    if (const char *e = getenv("TGB_ANALYTIC_BVH_MIN")) analytic_bvh_min = size_t(std::max(1, atoi(e)));
-    const bool analytic_in_bvh = analytic.size() >= analytic_bvh_min;
-    std::vector<Aabb> abounds(analytic.size());
-    for (size_t k = 0; k < analytic.size(); ++k) abounds[k] = analytic_bounds(prims[size_t(analytic[k])]);
-    SceneBvhInput in;
-    in.tris = btris.data(); in.n_tris = uint32_t(btris.size());
-    in.curve_boxes = cboxes.data(); in.curve_recs = crecs.data(); in.n_curve = uint32_t(cboxes.size());
-    if (analytic_in_bvh) { in.analytic = abounds.data(); in.n_analytic = uint32_t(abounds.size()); }
-    in.extent = std::max(std::max(std::fabs(sc.cam.pos.x), std::fabs(sc.cam.pos.y)), std::fabs(sc.cam.pos.z));
-    SceneBvh sb;
-    build_scene_bvh(in, bvh_options(), sb);
-    const Bvh4 &bvh = sb.tree;
-    if (!cboxes.empty()) {
-        for (uint32_t pi : cseg_prim) tri_prim.push_back(pi);
-        for (DPrim &p : prims) if (p.type == TGB_PRIM_CURVES) p.tri_first += uint32_t(btris.size());
-    }
-    std::vector<int> analytic_loop = analytic;           // what the ray-creating kernels loop over
-    if (analytic_in_bvh)                                  // ... nothing: the list goes into BVH leaf order instead
-        for (size_t k = 0; k < sb.analytic_order.size(); ++k) analytic_loop[k] = analytic[sb.analytic_order[k]];
-    {   // ray-binning grid: bounds of every finite primitive (TraceableScene::_sceneBounds, TraceableScene.hpp:104-110)
-        float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
-        auto grow = [&](const float *p) { for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], p[a]); hi[a] = std::max(hi[a], p[a]); } };
-        if (!bvh.nodes.empty()) { grow(bvh.lo); grow(bvh.hi); }
-        for (const Aabb &b : abounds) { grow(b.lo); grow(b.hi); }
-        for (int a = 0; a < 3; ++a) if (!(hi[a] > lo[a])) { lo[a] = -1.0f; hi[a] = 1.0f; }
-        sc.bin_lo = v3(lo[0], lo[1], lo[2]);
-        sc.bin_inv = v3(16.0f/(hi[0] - lo[0]), 16.0f/(hi[1] - lo[1]), 16.0f/(hi[2] - lo[2]));
-    }
-    sc.n_cut = int(sb.cut.size());
-    for (int i = 0; i < sc.n_cut; ++i) {
-        for (int a = 0; a < 3; ++a) { sc.cut[2*a][i] = sb.cut[size_t(i)].lo[a]; sc.cut[2*a + 1][i] = sb.cut[size_t(i)].hi[a]; }
-        sc.cut_link[i] = sb.cut[size_t(i)].link;
-    }
-    {
-        const char *e = getenv("TGB_SHADOW_CUT_ENTRY");
-        sc.cut_entry = (e && e[0] == '0') ? 0 : 1;
-    }
-    if (sb.stack_need > uint32_t(kStackSize)) return fail(c, TGB_ERR_UNSUPPORTED, "BVH depth %u (%u stack entries) exceeds the traversal stack", bvh.max_depth, sb.stack_need);
-    c->bvh_depth = bvh.max_depth; c->n_tris = uint32_t(btris.size()); c->bvh_sah = bvh.sah_cost;
-    c->geom_bytes = sb.qtree.nodes.size()*sizeof(QNode4) + sb.isect.size()*sizeof(IsectRecord) + tri_shade.size()*16 + bvh.order.size()*8;
-
-    int rc;
-    if ((rc = dev_upload(c, &sc.prims, prims))) return rc;
-    if ((rc = dev_upload(c, &sc.bsdfs, bsdfs))) return rc;
-    c->n_bsdfs = int(bsdfs.size());
-    c->prim_types.resize(prims.size());
-    for (size_t i = 0; i < prims.size(); ++i) c->prim_types[i] = prims[i].type;
-    c->light_ids = lights;
-    for (int li : lights) c->mesh_lights = c->mesh_lights || prims[size_t(li)].type == TGB_PRIM_MESH;
-    std::vector<uint32_t> slots(d->bsdf_slots, d->bsdf_slots + d->n_bsdf_slots);
-    if ((rc = dev_upload(c, &sc.slots, slots))) return rc;
-    if ((rc = dev_upload(c, &sc.tex, dtex))) return rc;
-    if ((rc = dev_upload(c, &sc.lights, lights))) return rc;
-    if ((rc = dev_upload(c, &sc.inf_lights, inf_lights))) return rc;
-    if ((rc = dev_upload(c, &sc.analytic, analytic_loop))) return rc;
-    if ((rc = dev_upload(c, &sc.tri_global, bvh.order))) return rc;
-    if ((rc = dev_upload(c, &sc.tri_prim, tri_prim))) return rc;
-    {   // shading records follow the intersection records into BVH leaf order (one hop from a hit id)
-        std::vector<float4> shade_leaf(tri_shade.size());
-        for (size_t k = 0; k < btris.size(); ++k) std::memcpy(&shade_leaf[4*k], &tri_shade[4*size_t(bvh.order[k])], 4*sizeof(float4));
-        if ((rc = dev_upload(c, &sc.tri_shade, shade_leaf))) return rc;
-    }
-    {
-        static_assert(sizeof(IsectRecord) == 3*sizeof(float4), "intersection record layout");
-        const IsectRecord *ir = nullptr;
-        if ((rc = dev_upload(c, &ir, sb.isect))) return rc;
-        sc.tri_isect = reinterpret_cast<const float4 *>(ir);
-    }
-    {
-        const QNode4 *qn = nullptr;
-        if ((rc = dev_upload(c, &qn, sb.qtree.nodes))) return rc;
-        sc.qnodes = reinterpret_cast<const uint4 *>(qn); sc.qy = 0x3F80u;
-    }
-    {   // the direction matrices, then per dimension the XOR of the columns of every low byte (sampler_next1d): 1 MiB
-        std::vector<uint32_t> sobol(size_t(kSobolLowTable) + size_t(kSobolDims)*256);
-        std::memcpy(sobol.data(), tgb_sobol_blob, size_t(kSobolLowTable)*4);
-        for (uint32_t dim = 0; dim < kSobolDims; ++dim) {
-            const uint32_t *m = sobol.data() + dim*32u;
-            uint32_t *lo = sobol.data() + kSobolLowTable + dim*256u;
-            lo[0] = 0u;
-            for (uint32_t b = 1; b < 256; ++b) lo[b] = lo[b & (b - 1)] ^ m[__builtin_ctz(b)];
-        }
-        if ((rc = dev_upload(c, &sc.sobol, sobol))) return rc;
-    }
-    sc.n_prims = uint32_t(prims.size()); sc.n_lights = int(lights.size()); sc.n_inf_lights = int(inf_lights.size());
-    sc.n_analytic = analytic_in_bvh ? 0 : int(analytic.size()); sc.analytic_base = analytic_in_bvh ? int(sb.isect.size()) : 0x7fffffff;
-    sc.n_nodes = uint32_t(bvh.nodes.size()); sc.n_tris = uint32_t(btris.size());
-    sc.n_curve_segs = uint32_t(cboxes.size()); c->has_curves = !cboxes.empty();
-    {
-        uint32_t types = 0;
-        for (uint32_t i = 0; i < d->n_primitives; ++i) {
-            const tgb_primitive &p = d->primitives[i];
-            if (p.type == TGB_PRIM_INFINITE_SPHERE || p.type == TGB_PRIM_INFINITE_SPHERE_CAP || p.type == TGB_PRIM_SKYDOME) continue;
-            for (uint32_t k = 0; k < p.bsdf_count; ++k) {
-                uint32_t t = d->bsdfs[d->bsdf_slots[p.bsdf_first + k]].type;
-                if (t != TGB_BSDF_NULL) types |= 1u << std::min(t, 31u);
-            }
-        }
-        const char *env = getenv("TGB_SORT_MATERIALS");
-        c->sort_materials = env ? env[0] == '1' : __builtin_popcount(types) >= 2;
-        // every surface Lambert (lights: null BSDF): k_shade's lobe-set-1 instantiation (same arithmetic, a fraction of the code)
-        const char *ls = getenv("TGB_LOBE_SET");
-        c->diffuse_only = (types & ~(1u << TGB_BSDF_LAMBERT)) == 0 && !c->has_curves && !(ls && ls[0] == '0');
-        if (c->diffuse_only) c->sort_materials = false;
-        // ... and every light a quad, no infinite emitter, every BSDF albedo and emission texture constant: the emitter-set-1
-        // instantiation of it (k_shade<false, false, 1, 1>: the same arithmetic without the other emitters' and textures' code)
-        bool quads = c->diffuse_only && inf_lights.empty() && TGB_QUAD_EMITTERS;
-        for (int li : lights) quads = quads && prims[size_t(li)].type == TGB_PRIM_QUAD;
-        for (const DPrim &p : prims) quads = quads && (p.emission_tex < 0 || dtex[size_t(p.emission_tex)].type == TGB_TEX_CONSTANT);
-        for (const DBsdf &b : bsdfs) quads = quads && (b.type != TGB_BSDF_LAMBERT || dtex[size_t(b.albedo_tex)].type == TGB_TEX_CONSTANT);
-        c->quad_emitters = quads;
-        if (quads) {    // its BSDFs as 16-byte records: constant albedo, type | lobes << 16 (lambert_rec)
-            std::vector<float4> lam(bsdfs.size());
-            for (size_t i = 0; i < bsdfs.size(); ++i) {
-                const DBsdf &b = bsdfs[i];
-                const V3 a = dtex[size_t(b.albedo_tex)].value;
-                const uint32_t w = (b.type & 0xFFFFu) | (b.lobes << 16);
-                float wf; std::memcpy(&wf, &w, 4);
-                lam[i] = make_float4(a.x, a.y, a.z, wf);
-            }
-            if ((rc = dev_upload(c, &sc.lambert, lam))) return rc;
-        }
-    }
-    return TGB_OK;
-}
-
-// The kernel instantiations of upload_scene's flags.  k_shade: material-sorted, then with curves, then the emitter set, then
-// Lambert-only, then the generic one.
-Kernels select_kernels(const tgb_ctx *c) {
-    const bool cv = c->has_curves;
+// The kernel instantiations of a scene.  k_shade: material-sorted (>= 2 lobe models in use, or TGB_SORT_MATERIALS=1; =0 never),
+// then with curves, then the emitter set, then Lambert-only (TGB_LOBE_SET=0 turns the last two off), then the generic one.
+Kernels select_kernels(const SceneKind &s) {
+    const bool cv = s.has_curves;
+    // every surface Lambert (lights: null BSDF): k_shade's lobe-set-1 instantiation (same arithmetic, a fraction of the code)
+    const char *ls = getenv("TGB_LOBE_SET"), *sm = getenv("TGB_SORT_MATERIALS");
+    const bool diffuse_only = (s.bsdf_types & ~(1u << TGB_BSDF_LAMBERT)) == 0 && !cv && !(ls && ls[0] == '0');
+    const bool sort_materials = !diffuse_only && (sm ? sm[0] == '1' : __builtin_popcount(s.bsdf_types) >= 2);
+    // ... and every light a quad, no infinite emitter, every BSDF albedo and emission texture constant: the emitter-set-1
+    // instantiation of it (k_shade<false, false, 1, 1>: the same arithmetic without the other emitters' and textures' code)
+    const bool quad_emitters = diffuse_only && s.quad_lights && TGB_QUAD_EMITTERS;
     Kernels k;
     k.trace = cv ? k_trace<true> : k_trace<false>;
-    if (c->sort_materials) {
+    if (sort_materials) {
         k.shade = cv ? k_shade<true, true> : k_shade<false, true>;
         k.shade_block = kShadeSortBlock; k.shade_paths = kShadeSortBlock*kShadeSortItems;
     } else {
-        k.shade = cv ? k_shade<true, false> : c->quad_emitters ? k_shade<false, false, 1, 1> : c->diffuse_only ? k_shade<false, false, 1> : k_shade<false, false>;
+        k.shade = cv ? k_shade<true, false> : quad_emitters ? k_shade<false, false, 1, 1> : diffuse_only ? k_shade<false, false, 1> : k_shade<false, false>;
         k.shade_block = 128; k.shade_paths = 128;
     }
     k.shadow_prep = cv ? k_shadow_prep<true> : k_shadow_prep<false>;
-    k.shadow_bvh = cv ? (c->mesh_lights ? k_shadow_bvh<true, true> : k_shadow_bvh<true, false>)
-                      : (c->mesh_lights ? k_shadow_bvh<false, true> : k_shadow_bvh<false, false>);
+    k.shadow_bvh = cv ? (s.mesh_lights ? k_shadow_bvh<true, true> : k_shadow_bvh<true, false>)
+                      : (s.mesh_lights ? k_shadow_bvh<false, true> : k_shadow_bvh<false, false>);
     k.hook_persist = cv ? k_hook_persist<true> : k_hook_persist<false>;
+    k.variant[0] = cv; k.variant[1] = sort_materials; k.variant[2] = diffuse_only; k.variant[3] = quad_emitters;
     return k;
+}
+
+// The only function that puts scene data on the device: a prepared scene's arrays, and the records that point to them
+int upload_scene(tgb_ctx *c, const HostScene &hs, const Kernels &ks) {
+    DScene &sc = c->sc;
+    sc = hs.sc;
+    int rc;
+    std::vector<DTex> dtex(hs.tex.size());
+    for (size_t i = 0; i < hs.tex.size(); ++i) {
+        const HostTex &t = hs.tex[i]; DTex &o = dtex[i] = t.d;
+        if (o.type == TGB_TEX_BITMAP && (rc = dev_upload(c, &o.texels, t.texels))) return rc;
+        if (t.has_dist) {
+            if ((rc = dev_upload(c, &o.marg_pdf, t.marg_pdf))) return rc;
+            if ((rc = dev_upload(c, &o.marg_cdf, t.marg_cdf))) return rc;
+            if ((rc = dev_upload(c, &o.pdf, t.pdf))) return rc;
+            if ((rc = dev_upload(c, &o.cdf, t.cdf))) return rc;
+        }
+    }
+    std::vector<DBsdf> bsdfs = hs.bsdfs;
+    for (size_t i = 0; i < bsdfs.size(); ++i) {
+        if (bsdfs[i].type != TGB_BSDF_HAIR) continue;
+        for (int p = 0; p < 3; ++p) {
+            const HairLobeTables &l = hs.hair[i].lobe[p];
+            if ((rc = dev_upload(c, &bsdfs[i].hair_table[p], l.table))) return rc;
+            if ((rc = dev_upload(c, &bsdfs[i].hair_pdfs[p], l.pdfs))) return rc;
+            if ((rc = dev_upload(c, &bsdfs[i].hair_cdfs[p], l.cdfs))) return rc;
+            if ((rc = dev_upload(c, &bsdfs[i].hair_sums[p], l.sums))) return rc;
+        }
+    }
+    std::vector<DPrim> prims = hs.prims;
+    for (const MeshLight &m : hs.mesh_lights) {
+        DPrim &o = prims[m.prim];
+        if ((rc = dev_upload(c, &o.tri_pdf, m.pdf))) return rc;
+        if ((rc = dev_upload(c, &o.tri_cdf, m.cdf))) return rc;
+        if ((rc = dev_upload(c, &o.light_verts, m.verts))) return rc;
+    }
+    if ((rc = dev_upload(c, &sc.prims, prims))) return rc;
+    if ((rc = dev_upload(c, &sc.bsdfs, bsdfs))) return rc;
+    if ((rc = dev_upload(c, &sc.slots, hs.slots))) return rc;
+    if ((rc = dev_upload(c, &sc.tex, dtex))) return rc;
+    if ((rc = dev_upload(c, &sc.lights, hs.lights))) return rc;
+    if ((rc = dev_upload(c, &sc.inf_lights, hs.inf_lights))) return rc;
+    if ((rc = dev_upload(c, &sc.analytic, hs.analytic))) return rc;
+    if ((rc = dev_upload(c, &sc.tri_global, hs.bvh.tree.order))) return rc;
+    if ((rc = dev_upload(c, &sc.tri_prim, hs.tri_prim))) return rc;
+    if ((rc = dev_upload(c, &sc.tri_shade, hs.tri_shade))) return rc;
+    static_assert(sizeof(IsectRecord) == 3*sizeof(float4), "intersection record layout");
+    const IsectRecord *ir = nullptr;
+    if ((rc = dev_upload(c, &ir, hs.bvh.isect))) return rc;
+    sc.tri_isect = reinterpret_cast<const float4 *>(ir);
+    const QNode4 *qn = nullptr;
+    if ((rc = dev_upload(c, &qn, hs.bvh.qtree.nodes))) return rc;
+    sc.qnodes = reinterpret_cast<const uint4 *>(qn);
+    if ((rc = dev_upload(c, &sc.sobol, hs.sobol))) return rc;
+    if (ks.variant[3]) {    // the emitter-set k_shade reads its BSDFs as 16-byte records: constant albedo, type | lobes << 16 (lambert_rec)
+        std::vector<float4> lam(bsdfs.size());
+        for (size_t i = 0; i < bsdfs.size(); ++i) {
+            const DBsdf &b = bsdfs[i];
+            const V3 a = dtex[size_t(b.albedo_tex)].value;
+            const uint32_t w = (b.type & 0xFFFFu) | (b.lobes << 16);
+            float wf; std::memcpy(&wf, &w, 4);
+            lam[i] = make_float4(a.x, a.y, a.z, wf);
+        }
+        if ((rc = dev_upload(c, &sc.lambert, lam))) return rc;
+    }
+    // host copies for the test hooks and tgb200_scene_info
+    c->res_x = sc.cam.res_x; c->res_y = sc.cam.res_y;
+    c->has_curves = hs.kind.has_curves;
+    c->n_bsdfs = int(bsdfs.size());
+    c->prim_types.resize(prims.size());
+    for (size_t i = 0; i < prims.size(); ++i) c->prim_types[i] = prims[i].type;
+    c->light_ids = hs.lights;
+    const Bvh4 &bvh = hs.bvh.tree;
+    c->bvh_depth = bvh.max_depth; c->n_tris = sc.n_tris; c->bvh_sah = bvh.sah_cost;
+    c->geom_bytes = hs.bvh.qtree.nodes.size()*sizeof(QNode4) + hs.bvh.isect.size()*sizeof(IsectRecord) + hs.tri_shade.size()*16 + bvh.order.size()*8;
+    return TGB_OK;
 }
 
 int alloc_wavefront(tgb_ctx *c, uint32_t capacity) {
@@ -1151,9 +704,8 @@ int group_render(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_
     return TGB_OK;
 }
 
-int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
-    tgb_ctx *c = nullptr;
-    *out = nullptr;
+// The settings a scene is refused for before it is prepared
+int check_settings(const tgb_scene_desc *d) {
     if (d->abi_version != TGB200_ABI_VERSION) return fail(nullptr, TGB_ERR_INVALID, "ABI version mismatch (got %u, library is %u)", d->abi_version, TGB200_ABI_VERSION);
     if (!d->settings.use_sobol) return fail(nullptr, TGB_ERR_UNSUPPORTED, "only the Sobol sampler (renderer.stratified_sampler = true) is on the hot path");
     if (d->settings.supplemental_mode != 0) return fail(nullptr, TGB_ERR_UNSUPPORTED, "supplemental_mode %u: the per-tile serial PCG stream cannot be reproduced by a wavefront renderer (DESIGN.md section 3)", d->settings.supplemental_mode);
@@ -1161,9 +713,15 @@ int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
     // max_bounces 0: PathTracer::traceSample's loop never runs and every sample is black; the wavefront's first shade would add
     // bounce-0 emission, so the setting is refused rather than rendered differently
     if (d->settings.max_bounces > 255 || d->settings.max_bounces < 1) return fail(nullptr, TGB_ERR_UNSUPPORTED, "max_bounces must be in [1, 255]");
+    return TGB_OK;
+}
+
+// A context for a prepared scene on device dev (< 0: the current device)
+int create_single(const HostScene &hs, int dev, tgb_ctx **out) {
+    tgb_ctx *c = nullptr;
+    *out = nullptr;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(nullptr, TGB_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU fallback)"); }
-    int dev = d->settings.device;
     if (dev < 0) { if (cudaGetDevice(&dev) != cudaSuccess) dev = 0; }
     if (dev >= ndev) return fail(nullptr, TGB_ERR_NO_DEVICE, "CUDA device %d not present (%d devices)", dev, ndev);
     cudaDeviceProp prop;
@@ -1184,10 +742,11 @@ int create_single(const tgb_scene_desc *d, tgb_ctx **out) {
                 cudaEventCreateWithFlags(&w.ev_ring[k], cudaEventDisableTiming);
                 for (cudaEvent_t &e : w.ev_k[k]) cudaEventCreate(&e);
             }
-        if ((rc = upload_scene(c, d))) break;
-        c->ks = select_kernels(c);
+        c->ks = select_kernels(hs.kind);
+        if ((rc = upload_scene(c, hs, c->ks))) break;
         // default: 2 x 4 Mi paths in flight (H100, C1: 2 x 2 Mi measured 3 % slower)
-        uint32_t cap = d->settings.max_paths_in_flight ? d->settings.max_paths_in_flight : (1u << 23);
+        const uint32_t max_paths = hs.sc.set.max_paths_in_flight;
+        uint32_t cap = max_paths ? max_paths : (1u << 23);
         cap = std::max(cap, 1024u);
         if ((rc = alloc_wavefront(c, cap))) break;
         {   // persistent traversal grid of one wavefront: what is resident at once (blocks per SM x SMs, smaller of the two
@@ -1394,21 +953,19 @@ int tgb200_create(const tgb_scene_desc *d, tgb_ctx **out) {
     if (!d || !out) return fail(nullptr, TGB_ERR_INVALID, "null argument");
     *out = nullptr;
     const uint32_t N = d->settings.n_devices;
-    if (N <= 1) {
-        tgb_scene_desc one = *d;
-        if (N == 1) one.settings.device = d->settings.devices[0];
-        one.settings.n_devices = 0;
-        return create_single(&one, out);
-    }
     if (N > 8) return fail(nullptr, TGB_ERR_INVALID, "at most 8 devices");
     for (uint32_t i = 0; i < N; ++i) for (uint32_t j = 0; j < i; ++j)
         if (d->settings.devices[i] == d->settings.devices[j]) return fail(nullptr, TGB_ERR_INVALID, "device %d listed twice", d->settings.devices[i]);
-    // one context per GPU, created concurrently (each uploads its own replica of the scene; the host BVH build runs per member)
+    // the scene is checked and prepared once, before any device is touched
+    if (int rc = check_settings(d)) return rc;
+    HostScene hs;
+    if (int rc = prepare_scene(d, hs)) return rc;
+    if (N <= 1) return create_single(hs, N == 1 ? d->settings.devices[0] : d->settings.device, out);
+    // one context per GPU, created concurrently, each uploading the same prepared scene
     std::vector<tgb_ctx *> members(N, nullptr); std::vector<int> rcs(N, TGB_OK); std::vector<std::string> errs(N);
     std::vector<std::thread> th;
     for (uint32_t k = 0; k < N; ++k) th.emplace_back([&, k] {
-        tgb_scene_desc one = *d; one.settings.device = d->settings.devices[k]; one.settings.n_devices = 0;
-        rcs[k] = create_single(&one, &members[k]);
+        rcs[k] = create_single(hs, d->settings.devices[k], &members[k]);
         if (rcs[k]) errs[k] = g_create_error;
     });
     for (std::thread &t : th) t.join();
@@ -2088,8 +1645,7 @@ int tgb200_bin_probe(tgb_ctx *c, uint32_t n, const uint32_t *keys, uint32_t *ord
 
 int tgb200_shade_variant(const tgb_ctx *c, uint32_t *variant) {
     if (!c || !variant) return TGB_ERR_INVALID;
-    variant[0] = c->has_curves ? 1u : 0u; variant[1] = c->sort_materials ? 1u : 0u; variant[2] = c->diffuse_only ? 1u : 0u;
-    variant[3] = c->quad_emitters ? 1u : 0u;
+    std::memcpy(variant, c->ks.variant, sizeof(c->ks.variant));
     return TGB_OK;
 }
 
