@@ -60,6 +60,8 @@ int      oracle_shadow_probe(oracle_scene *s, int n, const float *query, const i
  * record's seed, the input of bounce 0 (only PIXEL, SEED and SAMPLE are read).  Returns -1 (nothing written) when a state to
  * step has bounce >= maxBounces. */
 int      oracle_bounce_probe(oracle_scene *s, int camera, int n, const uint32_t *in, uint32_t *out);
+/* Each segment of curve primitive prim on its own, for each ray: 7 words (see pt_oracle.c).  -1 when prim is not a curve. */
+int      oracle_curve_segments_probe(oracle_scene *s, int prim, const tgb_ray *rays, const int *only, int n, uint32_t *out);
 int      oracle_hair_eval(float roughness, float scale_angle_deg, const float *sigma_a, const float *wi_wo, int n, float *out);
 int      oracle_hair_tables(float roughness, float scale_angle_deg, const float *sigma_a, float *tables, float *sums, float *v);
 

@@ -59,6 +59,8 @@ def lib():
         L.oracle_shadow_probe.argtypes = [vp, C.c_int, vp, vp, vp]
         L.oracle_bounce_probe.restype = C.c_int
         L.oracle_bounce_probe.argtypes = [vp, C.c_int, C.c_int, vp, vp]
+        L.oracle_curve_segments_probe.restype = C.c_int
+        L.oracle_curve_segments_probe.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp]
         _LIB = L
     return _LIB
 
@@ -124,6 +126,26 @@ class Oracle:
         if rc != 0:
             raise RuntimeError("oracle_bounce_probe -> %d" % rc)
         return out
+
+    def curve_segments(self, prim, rays, only=None):
+        """oracle_curve_segments_probe: every segment of curve primitive `prim` tested alone on each ray (only: int [n], one
+        segment per ray, -1 = all).  Returns a record array: n_pass (segments whose root piece passes its box test), n_hit
+        (segments that report a hit), seg / t / u / w of the nearest such hit (seg -1: none), slack (where the hit point lies in
+        the segment's curveBox, in units of the box's largest extent: > 0 inside)."""
+        rays = np.ascontiguousarray(rays, dtype=np.float32).reshape(-1, 8)
+        out = np.zeros(len(rays), CURVE_SEGMENTS_DTYPE)
+        if only is not None:
+            only = np.ascontiguousarray(only, dtype=np.int32)
+            assert only.shape == (len(rays),)
+        rc = lib().oracle_curve_segments_probe(self.h, prim, rays.ctypes.data, None if only is None else only.ctypes.data,
+                                               len(rays), out.ctypes.data)
+        if rc != 0:
+            raise RuntimeError("oracle_curve_segments_probe: primitive %d is not a curve" % prim)
+        return out
+
+
+CURVE_SEGMENTS_DTYPE = np.dtype([("n_pass", "<u4"), ("n_hit", "<u4"), ("seg", "<i4"), ("t", "<f4"), ("u", "<f4"), ("w", "<f4"),
+                                 ("slack", "<f4")])
 
 
 def kat_eval(which, args):

@@ -15,12 +15,15 @@ Comparison (stated here, used below):
   * status, bounce, wasSpecular, sampler dimension and PCG state: exactly equal.  The exceptions are classed per path and each
     class is a row of EXCEPTIONS with its reason and the count an H100 run measured (seeded inputs: the same count every run):
       - hit tie: the two closest-hit implementations (tgb200_trace_closest and the oracle's) pick different primitives for the
-        path's ray -- coplanar or touching surfaces, as test_gpu_shadow.py classes its ties;
+        path's ray -- coplanar or touching surfaces, as test_gpu_shadow.py classes its ties -- or, on overlapping curve segments,
+        different segments or the same segment at a different t;
       - flip: a discrete decision of the bounce differs although the ray is the same; the inputs of that decision differ by a
         few ulp (libm on the device against glibc: a BSDF's sin / cos / exp / pow), which moves the decision only when it sits
         on its edge;
       - NaN throughput: the one place where the NaN rule of k_shade / k_accum and traceSample's differ (see _NAN_THR);
-  * origin, tmin, direction, throughput and radiance: within per-scene ulp bars (ulp of the largest component of the vector),
+  * origin and tmin: exact outside the classes above (the curve epsilon, 0.1 x width on `cylinder` curves and 0.01 x width
+    otherwise, moves tmin);
+  * direction, throughput and radiance: within per-scene ulp bars (ulp of the largest component of the vector),
     3x what an H100 run measured, except paths of the classes above and paths whose direct-light estimate differs grossly
     (> 2^16 ulp: a shadow query that grazes a silhouette decided the other way), which are counted in the "flip" rows too.
 Every run prints what it measured.  Each edge stratum also asserts that its case happened: roulette killed some paths and kept
@@ -40,6 +43,11 @@ Which scene runs which k_shade instantiation (KSHADE below is checked against th
     many_lights        <false, false, 1>               39 samplable lights (> 16)
     cube_city          <false, false, 1>               analytic primitives in BVH leaves
     hair_sky           <true, true, 0>                 the shipped hair scene's sphere cap (sampled) + skydome (not sampled)
+    curves_cylinder    <true, false, 0>                `cylinder` curves (Lambert, curve_taper, curve_thickness): the localP
+                                                       normal and the 0.1 x width curve epsilon
+    curves_half_cyl    <true, true, 0>                 `half_cylinder` curves (rough plastic, subsample): the localP normal and
+                                                       the 0.01 x width curve epsilon (widths 0.043-0.10: on most strands
+                                                       0.01 x width is above the 5e-4 floor it is the max of)
 """
 import os
 
@@ -65,16 +73,20 @@ EXACT = [abi.BR_BOUNCE, abi.BR_FLAGS, abi.BR_DIMENSION, abi.BR_PCG, abi.BR_PCG +
 KSHADE = {"cornell_box": "<false, false, 1>", "cornell_mesh": "<false, false, 1>", "cornell_generic": "<false, false, 0>",
           "materials_env": "<false, true, 0>", "dirac_room": "<false, true, 0>", "coat_room": "<false, true, 0>",
           "hair_scene": "<true, true, 0>", "hair_unsorted": "<true, false, 0>", "many_lights": "<false, false, 1>",
-          "cube_city": "<false, false, 1>", "hair_sky": "<true, true, 0>"}
+          "cube_city": "<false, false, 1>", "hair_sky": "<true, true, 0>", "curves_cylinder": "<true, false, 0>",
+          "curves_half_cyl": "<true, true, 0>"}
 
 # (stratum, class) -> (paths, reason), measured on an H100 80GB HBM3 at a 700 W power limit over all bounces of the stratum
 _TIE_CURVES = ("the closest hits of tgb200_trace_closest and the oracle differ for the path's ray: overlapping curve segments, which "
-               "the two BVHs test in different orders (DESIGN.md section 2)")
+               "the two BVHs test in different orders, so a segment is entered with another tmax and prunes other pieces (DESIGN.md "
+               "section 2, tests/test_gpu_curve_hits.py's multi class)")
 _TIE = "the closest hits of tgb200_trace_closest and the oracle differ for the path's ray: touching or coplanar surfaces"
 _FLIP_LIGHT = ("ray, next ray and sampler state agree, only the direct light differs: a shadow query or a light choice among 39 "
                "lights decided the other way on a light-sample direction a few ulp apart")
 _FLIP_HAIR = ("same status, direction and sampler state, a different throughput: the hair BCSDF's table cell, chosen from a "
               "libm result a few ulp apart")
+_FLIP_CURVES = ("same status, ray and sampler state, a finished radiance far apart: a discrete part of the direct-light estimate "
+                "(a shadow query grazing one of the wide, overlapping strands) decided the other way")
 _NAN_THR = ("NaN throughput on a bounce that issues no shadow query: the reference adds the zero direct-light estimate times the "
             "throughput (NaN, and no NaN guard follows when the BSDF sample then fails); k_shade adds nothing.  A render never starts "
             "a bounce with a NaN throughput (k_accum ends such paths); an infinite one passes the guard (DESIGN.md)")
@@ -82,7 +94,9 @@ EXCEPTIONS = {("hair_scene", "hit tie"): (82, _TIE_CURVES), ("hair_unsorted", "h
               ("hair_sky", "hit tie"): (63, _TIE_CURVES), ("hair_sky misses", "hit tie"): (15, _TIE_CURVES),
               ("hair_sky misses", "flip"): (1, _FLIP_HAIR),
               ("many_lights", "hit tie"): (2, _TIE), ("many_lights", "flip"): (6, _FLIP_LIGHT),
-              ("cornell_box edges", "NaN throughput"): (54, _NAN_THR)}
+              ("cornell_box edges", "NaN throughput"): (54, _NAN_THR),
+              ("curves_cylinder", "hit tie"): (4, _TIE_CURVES), ("curves_half_cyl", "hit tie"): (102, _TIE_CURVES),
+              ("curves_half_cyl", "flip"): (1, _FLIP_CURVES)}
 
 # stratum -> (origin + tmin, direction, throughput, emission of survivors, radiance of finished paths) ulp bars: 3x what an H100 run
 # measured (in the comment), at most GROSS_ULP: past it a path counts as a flip, so GROSS_ULP is the bar where 3x would exceed it.
@@ -100,6 +114,8 @@ ULP_BARS = {
     "many_lights":                     (0, 6, 0, GROSS_ULP, GROSS_ULP),  # measured (0, 2, 0, 36790, 18650): 3x is past the cutoff
     "cube_city":                       (0, 6, 0, 19533, 7818),  # measured (0, 2, 0, 6511, 2606)
     "hair_sky":                        (0, 504, 426, 144, 999),  # measured (0, 167.8, 142, 48, 333)
+    "curves_cylinder":                 (0, 6, 0, 2517, 420),  # measured (0, 2, 0, 839, 140)
+    "curves_half_cyl":                 (0, 12, 2193, 2517, 498),  # measured (0, 4, 731, 839, 166)
     "cornell_box min_bounces_2":       (0, 6, 0, 6, 0),  # measured (0, 2, 0, 2, 0)
     "cornell_box max_bounces_2":       (0, 6, 0, 0, 0),  # measured (0, 2, 0, 0, 0)
     "cornell_box no_nee":              (0, 6, 0, 0, 0),  # measured (0, 2, 0, 0, 0)
@@ -178,14 +194,16 @@ def compare(ctx, orc, states, tally):
     u[alive, 3] = _vec_ulp(fl(g, EMI)[alive], fl(r, EMI)[alive])
     u[done, 4] = _vec_ulp(fl(g, EMI)[done], fl(r, EMI)[done])
     gross = ~bad & (u > GROSS_ULP).any(1)
-    odd = bad | gross
+    # origin and tmin are exact unless the two walks found different hits for the path's ray (same segment at another t included)
+    odd = bad | gross | (u[:, 0] > 0)
     if odd.any():
         idx = np.flatnonzero(odd)
         rays = np.zeros((len(idx), 8), F)
         rays[:, :3] = fl(states, ORIGIN)[idx]; rays[:, 3:6] = fl(states, DIR)[idx]; rays[:, 6] = fl(states, [abi.BR_TMIN])[idx, 0]
         rays[:, 7] = np.inf
         hg, hr = ctx.trace_closest(rays), orc.trace(rays)
-        tie = (hg["primitive"] != hr["primitive"]) | ((hg["primitive"] >= 0) & (hg["prim_id"] != hr["prim_id"]))
+        tie = (hg["primitive"] != hr["primitive"]) | ((hg["primitive"] >= 0) & ((hg["prim_id"] != hr["prim_id"]) |
+                                                                               (hg["t"].view(np.uint32) != hr["t"].view(np.uint32))))
         for j, i in enumerate(idx):
             cls = "hit tie" if tie[j] else "NaN throughput" if np.isnan(fl(states, THR)[i]).any() else "flip"
             tally.counts[cls] = tally.counts.get(cls, 0) + 1
@@ -239,6 +257,14 @@ def make_scene(name, scratch, monkeypatch=None, **kw):
         return scene.load_scene(synth.many_lights(scratch, name="bounce_ml", res=(32, 32), spp=1, subdiv=3))
     if name == "cube_city":
         return scene.load_scene(synth.cube_city(res=(32, 32), spp=1, n=12))
+    if name == "curves_cylinder":           # test_gpu_parity.test_curves_and_hair's two non-hair modes, at probe size (the
+                                            # half_cylinder strands wider, so that their epsilon is not the 5e-4 floor)
+        return scene.load_scene(synth.hair_scene(scratch, name="bounce_cyl", n_curves=300, res=(32, 32), spp=1, mode="cylinder",
+                                                 bsdf={"type": "lambert", "albedo": [0.6, 0.4, 0.2]}, thickness=0.015, taper=True))
+    if name == "curves_half_cyl":
+        return scene.load_scene(synth.hair_scene(scratch, name="bounce_half_cyl", n_curves=300, res=(32, 32), spp=1,
+                                                 mode="half_cylinder", bsdf={"type": "rough_plastic", "albedo": [0.6, 0.4, 0.2],
+                                                                             "roughness": 0.2}, subsample=0.3, width=0.07))
     return scene.load_scene(os.path.join(G, name, "scene.json"))          # materials_env, hair_sky
 
 
@@ -251,6 +277,12 @@ def test_chained_bounces_match_oracle(name, scratch, monkeypatch):
     fs = make_scene(name, scratch, monkeypatch)
     ctx = lib.Context(fs); orc = pyoracle.Oracle(fs)
     assert ctx.shade_variant() == KSHADE[name]
+    if name.startswith("curves_"):          # the curve epsilon max(5e-4, k x width) is k x width on most strands
+        p = next(p for p in fs.primitives if p.type == abi.PRIM_CURVES)
+        w = np.ctypeslib.as_array(p.curve_nodes, shape=(p.n_curve_nodes*4,))[3::4]
+        k = F(0.1) if p.curve_mode == abi.CURVE_CYLINDER else F(0.01)
+        print("%s: %.3f of the nodes have k x width > 5e-4" % (name, float((k*w > F(5e-4)).mean())))
+        assert (k*w > F(5e-4)).mean() > 0.5
     tally = Tally(name)
     steps = chain(ctx, orc, camera_states(fs, orc, N_PATHS), tally)
     alive = [int((r[:, abi.BR_STATUS] == 1).sum()) for _, _, r in steps]

@@ -196,54 +196,12 @@ TGB_D void curve_half_cylinder(const CurvePiece &node, float tMin, float &tMax, 
     float newT = segmentT*(node.tMax - node.tMin) + node.tMin;
     if (newT >= 0.0f && newT <= 1.0f) { hu = newT; ht = t0; hw = width; tMax = t0; }
 }
-// pointOnSpline<false>: p0..p2 are the projected nodes; true when a hit closer than tMax was found (t, u, w are set).
-// The reference keeps an explicit stack of pieces (tMin, tMax, both end points).  Every end point is the same function of its
-// dyadic parameter (q0*t*t + q1*t + q2, t = k/2^depth, exact in float), and the stack is strictly LIFO with one pending sibling
-// per depth, so the stack is a 5-bit mask here and a popped piece's end points are re-evaluated: same values, same visiting
-// order, no local-memory traffic (the 5 x 44-byte stack was the kernel's only local array).
+// pointOnSpline<false> runs in bvh_traverse_persistent's BISECT / CYL states.  The reference keeps an explicit stack of pieces
+// (tMin, tMax, both end points).  Every end point is the same function of its dyadic parameter (q0*t*t + q1*t + q2, t = k/2^depth,
+// exact in float), and the stack is strictly LIFO with one pending sibling per depth, so the stack is a 5-bit mask there and a
+// popped piece's end points are re-evaluated with curve_eval: same values, same visiting order, no local-memory traffic.
 TGB_D float4 curve_eval(float4 q0, float4 q1, float4 q2, float t) {
     return f4add(f4add(f4scale(q0, t*t), f4scale(q1, t)), q2);
-}
-TGB_D bool curve_point_on_spline(float4 p0, float4 p1, float4 p2, float tMin, float tMax, float &ht, float &hu, float &hw) {
-    constexpr int MaxDepth = 5;
-    float4 q0 = f4add(f4sub(f4scale(p0, 0.5f), p1), f4scale(p2, 0.5f));
-    float4 q1 = f4sub(p1, p0);
-    float4 q2 = f4scale(f4add(p0, p1), 0.5f);
-    float tFlatX = -q1.x*0.5f/q0.x, tFlatY = -q1.y*0.5f/q0.y;
-    float xFlat = q0.x*tFlatX*tFlatX + q1.x*tFlatX + q2.x;
-    float yFlat = q0.y*tFlatY*tFlatY + q1.y*tFlatY + q2.y;
-    CurvePiece cur; cur.p0 = q2; cur.p1 = f4add(f4add(q0, q1), q2); cur.tMin = 0.0f; cur.tMax = 1.0f; cur.depth = 0;
-    uint32_t idx = 0, pending = 0;                 // the piece is [idx, idx + 1]/2^depth; bit L of pending = the sibling at depth L waits
-    float closestDepth = tMax;
-    for (;;) {
-        float pMinX = cur.p1.x < cur.p0.x ? cur.p1.x : cur.p0.x, pMinY = cur.p1.y < cur.p0.y ? cur.p1.y : cur.p0.y;
-        float pMaxX = cur.p1.x > cur.p0.x ? cur.p1.x : cur.p0.x, pMaxY = cur.p1.y > cur.p0.y ? cur.p1.y : cur.p0.y;
-        if (tFlatX > cur.tMin && tFlatX < cur.tMax) { pMinX = minf(pMinX, xFlat); pMaxX = maxf(pMaxX, xFlat); }
-        if (tFlatY > cur.tMin && tFlatY < cur.tMax) { pMinY = minf(pMinY, yFlat); pMaxY = maxf(pMaxY, yFlat); }
-        float maxWidth = maxf(cur.p0.w, cur.p1.w);
-        if (pMinX <= maxWidth && pMinY <= maxWidth && pMaxX >= -maxWidth && pMaxY >= -maxWidth) {
-            if (cur.depth >= MaxDepth) {
-                curve_half_cylinder(cur, tMin, closestDepth, ht, hu, hw);
-            } else {
-                float splitT = (cur.tMin + cur.tMax)*0.5f;
-                float4 qSplit = curve_eval(q0, q1, q2, splitT);
-                cur.depth = cur.depth + 1; pending |= 1u << cur.depth;
-                if (cur.p0.z < qSplit.z) { idx = 2*idx;     cur.tMax = splitT; cur.p1 = qSplit; }     // near half first, the other half waits
-                else                     { idx = 2*idx + 1; cur.tMin = splitT; cur.p0 = qSplit; }
-                continue;
-            }
-        }
-        do {
-            if (pending == 0) return closestDepth < tMax;
-            int L = 31 - __clz(pending); pending ^= 1u << L;
-            idx = (idx >> (cur.depth - L)) ^ 1u; cur.depth = L;
-            float scale = __uint_as_float(uint32_t(127 - L) << 23);                   // 2^-L
-            cur.tMin = float(idx)*scale; cur.tMax = float(idx + 1)*scale;
-            float4 e0 = curve_eval(q0, q1, q2, cur.tMin);
-            cur.p0 = idx == 0 ? q2 : e0;                                              // (the root's first end point is q2 itself)
-            cur.p1 = curve_eval(q0, q1, q2, cur.tMax);
-        } while (minf(cur.p0.z - cur.p0.w, cur.p1.z - cur.p1.w) > closestDepth);
-    }
 }
 // ---- BVH traversal ------------------------------------------------------------------------------
 // Traversal stack: the first kSmemStack entries of every lane live in shared memory, laid out [entry][thread] so that lane i
