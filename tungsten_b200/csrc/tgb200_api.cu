@@ -9,6 +9,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -22,20 +23,36 @@ using namespace tgb;
 #include <thread>
 #include <map>
 
-struct tgb_ctx;
-struct Group {
-    std::vector<tgb_ctx *> members;                     // members[0] = root
-    std::vector<tgb_tile> deal_key;                      // tile list the cached deal belongs to
-    std::vector<std::vector<tgb_tile>> shares;           // per member
-    std::vector<uint32_t *> root_pix;                    // per member k >= 1: its share's pixel ids on the ROOT device
-    std::vector<uint32_t> share_pixels;
-    std::vector<float4 *> send;                          // per member k >= 1: pack buffer on ITS device
-    float4 *recv = nullptr; size_t recv_capacity = 0;    // on the root device
-    std::vector<size_t> send_capacity;
-    double gather_ms = 0.0;
-};
-
 namespace {
+
+// A device array (Pinned: a page-locked host array) that frees itself; move-only.  ensure(n) re-allocates only when n exceeds
+// the capacity, and frees the old array first.  cudaFree waits for the device, so a kernel still queued that reads the old
+// array (k_resolve reading R) finishes before it goes.  After a failed allocation the buffer is empty.  upload(src, n, st):
+// ensure(n), then the host-to-device copy of n elements queued on st.
+template <typename T, bool Pinned = false>
+struct Buffer {
+    T *p = nullptr;
+    size_t cap = 0;
+    Buffer() = default;
+    Buffer(Buffer &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    ~Buffer() { release(); }
+    void release() {
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr; cap = 0;
+    }
+    cudaError_t ensure(size_t n) {
+        if (n <= cap) return cudaSuccess;
+        release();
+        void *q = nullptr;
+        const cudaError_t e = Pinned ? cudaMallocHost(&q, n*sizeof(T)) : cudaMalloc(&q, n*sizeof(T));
+        if (e == cudaSuccess) { p = static_cast<T *>(q); cap = n; }
+        return e;
+    }
+    cudaError_t upload(const T *src, size_t n, cudaStream_t st) {
+        const cudaError_t e = ensure(n);
+        return e != cudaSuccess || n == 0 ? e : cudaMemcpyAsync(p, src, n*sizeof(T), cudaMemcpyHostToDevice, st);
+    }
+};
 
 // One wavefront: the loop state of its share of a (sub)step's camera paths.  A context runs two of them, each on its own stream,
 // so that one wavefront's traversal kernels (ALU bound) run alongside the other's streaming kernels (HBM bound).
@@ -47,7 +64,7 @@ struct Wavefront {
     uint32_t *squeue_cl = nullptr;  // ... the closest-hit (mesh-light) queries left after the analytic pass
     uint32_t *bin_keys = nullptr, *bin_hist = nullptr;
     Ctl *ctl = nullptr;             // device-resident loop control block
-    Ctl *h_ctl = nullptr;           // pinned: [0..3] snapshot ring (read one iteration late), [4] initial value
+    Buffer<Ctl, true> h_ctl;        // [0..3] snapshot ring (read one iteration late), [4] initial value
     cudaEvent_t ev_ring[4]{};
     cudaEvent_t ev_k[4][8]{};       // profiling: boundaries between the kernels of an iteration (regen|trace|shade|prep|shadow|accum|sort)
 };
@@ -65,14 +82,35 @@ struct Kernels {
 
 }  // namespace
 
+struct tgb_ctx;
+// Multi-GPU (tgb_settings::devices): held by the root context; what it holds lives on the root's device
+struct Group {
+    explicit Group(std::vector<tgb_ctx *> m) : members(std::move(m)) {
+        for (cudaEvent_t &e : ev_gather) if (created == cudaSuccess) created = cudaEventCreate(&e);
+    }
+    ~Group() { for (cudaEvent_t e : ev_gather) if (e) cudaEventDestroy(e); }
+    std::vector<tgb_ctx *> members;                     // members[0] = root
+    std::vector<tgb_tile> deal_key;                      // tile list the cached deal belongs to
+    std::vector<std::vector<tgb_tile>> shares;           // per member
+    std::vector<Buffer<uint32_t>> root_pix;              // per member k >= 1: its share's pixel ids
+    std::vector<uint32_t> share_pixels;
+    Buffer<float4> recv;                                 // one member's packed share at a time
+    cudaEvent_t ev_gather[2] = {};
+    cudaError_t created = cudaSuccess;                   // the first error of the constructor's event creation
+    double gather_ms = 0.0;
+};
+
 struct tgb_ctx {
+    explicit tgb_ctx(int dev);      // on the current device, dev: the streams and events (created: the first error)
+    ~tgb_ctx();
     int device = 0;
+    cudaError_t created = cudaSuccess;
     cudaStream_t stream = nullptr;  // the caller's stream (tgb200_set_stream) or own_stream: wavefront 0, k_resolve, the hooks
     cudaStream_t stream1 = nullptr; // wavefront 1
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     std::string error;
     std::atomic<int> abort_flag{0};
-    std::vector<void *> allocs;
+    std::vector<Buffer<uint8_t>> arena;   // the allocations made once by tgb200_create (dev_alloc): scene, wavefronts, framebuffer
     DScene sc{};
     uint32_t res_x = 0, res_y = 0;
     // wavefront storage
@@ -83,23 +121,44 @@ struct tgb_ctx {
     bool has_curves = false;        // the probes pick their instantiations with the curve-segment test and per-hit epsilon
     Kernels ks;                     // the instantiations select_kernels chose for the scene
     int n_bsdfs = 0; std::vector<uint32_t> prim_types; std::vector<int> light_ids;   // host copies for the test hooks' argument checks
-    float4 *R = nullptr; size_t res_capacity = 0;   // finished radiance per path of the (sub)step
+    Buffer<float4> R;               // finished radiance per path of the (sub)step
     cudaStream_t own_stream = nullptr;
-    struct Group *group = nullptr;  // multi-GPU: set on the root context (devices[0]); members[0] == the root itself
-    Counters *ctr = nullptr; Counters *h_ctr = nullptr;
+    std::unique_ptr<Group> group;   // multi-GPU: set on the root context (devices[0]); members[0] == the root itself
+    Buffer<float4> send;            // multi-GPU member: its share's pixels packed for the gather on the root
+    Counters *ctr = nullptr; Buffer<Counters, true> h_ctr;
     float *fb = nullptr; uint32_t *fb_count = nullptr;
-    float *h_fb = nullptr; uint32_t *h_fb_count = nullptr;   // pinned staging
+    Buffer<float, true> h_fb; Buffer<uint32_t, true> h_fb_count;   // staging
     // cached pixel list
-    std::vector<tgb_tile> tiles_cached; uint32_t *pix_id = nullptr, *pix_seed = nullptr; uint32_t n_pix = 0, pix_capacity = 0;
+    std::vector<tgb_tile> tiles_cached; Buffer<uint32_t> pix_id, pix_seed; uint32_t n_pix = 0;
     std::vector<uint32_t> h_pix_id;                  // host copy of the pixel list (adaptive steps build per-pixel sample ranges from it)
     // adaptive sampling: per-pixel result-slot offsets / first sample index, pixel -> list index map, the 4x4 blocks' SampleRecords
-    uint32_t *pix_first = nullptr, *pix_base = nullptr, *pix_slot = nullptr; uint32_t adaptive_capacity = 0; bool pix_slot_valid = false;
-    SampleRecordD *rec_dev = nullptr;
+    Buffer<uint32_t> pix_first, pix_base, pix_slot; bool pix_slot_valid = false;
+    Buffer<SampleRecordD> rec_dev;
     tgb_stats stats{};
     bool profiling = false;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     uint32_t bvh_depth = 0; uint32_t n_tris = 0; double bvh_sah = 0.0; size_t geom_bytes = 0;
 };
+
+tgb_ctx::tgb_ctx(int dev) : device(dev) {
+    cudaError_t &e = created;
+    for (cudaStream_t *s : {&own_stream, &stream1}) if (e == cudaSuccess) e = cudaStreamCreateWithFlags(s, cudaStreamNonBlocking);
+    for (cudaEvent_t *v : {&ev0, &ev1}) if (e == cudaSuccess) e = cudaEventCreate(v);
+    for (cudaEvent_t *v : {&ev_fork, &ev_join}) if (e == cudaSuccess) e = cudaEventCreateWithFlags(v, cudaEventDisableTiming);
+    for (Wavefront &w : wf)
+        for (int k = 0; k < 4; ++k) {
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&w.ev_ring[k], cudaEventDisableTiming);
+            for (cudaEvent_t &v : w.ev_k[k]) if (e == cudaSuccess) e = cudaEventCreate(&v);
+        }
+    stream = own_stream;
+}
+
+tgb_ctx::~tgb_ctx() {
+    for (cudaEvent_t v : {ev0, ev1, ev_fork, ev_join}) if (v) cudaEventDestroy(v);
+    for (Wavefront &w : wf)
+        for (int k = 0; k < 4; ++k) { if (w.ev_ring[k]) cudaEventDestroy(w.ev_ring[k]); for (cudaEvent_t v : w.ev_k[k]) if (v) cudaEventDestroy(v); }
+    for (cudaStream_t s : {stream1, own_stream}) if (s) cudaStreamDestroy(s);
+}
 
 namespace {
 
@@ -115,10 +174,9 @@ int fail(tgb_ctx *c, int code, const char *fmt, ...) {
 
 template <typename T>
 int dev_alloc(tgb_ctx *c, T **out, size_t n) {
-    void *p = nullptr;
-    CU(cudaMalloc(&p, std::max<size_t>(n, 1)*sizeof(T)));
-    c->allocs.push_back(p);
-    *out = static_cast<T *>(p);
+    c->arena.emplace_back();
+    CU(c->arena.back().ensure(std::max<size_t>(n, 1)*sizeof(T)));
+    *out = reinterpret_cast<T *>(c->arena.back().p);
     return TGB_OK;
 }
 template <typename T>
@@ -259,18 +317,18 @@ int alloc_wavefront(tgb_ctx *c, uint32_t capacity) {
         if ((rc = dev_alloc(c, &w.bin_hist, size_t(kBins) + 4))) return rc;
         if ((rc = dev_alloc(c, &w.ctl, 1))) return rc;
         CU(cudaMemset(w.ctl, 0, sizeof(Ctl)));
-        CU(cudaMallocHost(reinterpret_cast<void **>(&w.h_ctl), 5*sizeof(Ctl)));
+        CU(w.h_ctl.ensure(5));
     }
     if ((rc = dev_alloc(c, &c->ctr, 1))) return rc;
     CU(cudaMemset(c->ctr, 0, sizeof(Counters)));
-    CU(cudaMallocHost(reinterpret_cast<void **>(&c->h_ctr), sizeof(Counters)));
+    CU(c->h_ctr.ensure(1));
     size_t npx = size_t(c->res_x)*c->res_y;
     if ((rc = dev_alloc(c, &c->fb, npx*3))) return rc;
     if ((rc = dev_alloc(c, &c->fb_count, npx))) return rc;
     CU(cudaMemset(c->fb, 0, npx*3*sizeof(float)));
     CU(cudaMemset(c->fb_count, 0, npx*sizeof(uint32_t)));
-    CU(cudaMallocHost(reinterpret_cast<void **>(&c->h_fb), npx*3*sizeof(float)));
-    CU(cudaMallocHost(reinterpret_cast<void **>(&c->h_fb_count), npx*sizeof(uint32_t)));
+    CU(c->h_fb.ensure(npx*3));
+    CU(c->h_fb_count.ensure(npx));
     return TGB_OK;
 }
 
@@ -317,19 +375,12 @@ int set_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t seed
     if (same_tiles(list, c->tiles_cached)) return TGB_OK;
     std::vector<uint32_t> pid, pseed;
     if (int rc = tile_pixels(c, list, pid, &pseed)) return rc;
-    if (pid.size() > c->pix_capacity) {
-        int rc;
-        if ((rc = dev_alloc(c, &c->pix_id, pid.size()))) return rc;
-        if ((rc = dev_alloc(c, &c->pix_seed, pid.size()))) return rc;
-        c->pix_capacity = uint32_t(pid.size());
-    }
+    c->tiles_cached.clear();                                    // (until the new list is on the device)
     c->n_pix = uint32_t(pid.size());
     c->h_pix_id = pid; c->pix_slot_valid = false;
-    if (c->n_pix) {
-        CU(cudaMemcpyAsync(c->pix_id, pid.data(), pid.size()*4, cudaMemcpyHostToDevice, c->stream));
-        CU(cudaMemcpyAsync(c->pix_seed, pseed.data(), pseed.size()*4, cudaMemcpyHostToDevice, c->stream));
-        CU(cudaStreamSynchronize(c->stream));
-    }
+    CU(c->pix_id.upload(pid.data(), pid.size(), c->stream));
+    CU(c->pix_seed.upload(pseed.data(), pseed.size(), c->stream));
+    CU(cudaStreamSynchronize(c->stream));
     c->tiles_cached = std::move(list);
     return TGB_OK;
 }
@@ -343,13 +394,9 @@ inline unsigned loop_grid(uint32_t resident, uint32_t bound) { return std::min(b
 // regeneration: whenever paths finish, their slots are refilled with the next camera paths of the step, so every
 // iteration traces a full batch until the step's paths run out (one drain tail per step instead of one per batch).
 int ensure_results(tgb_ctx *c, size_t n_paths) {
-    if (n_paths <= c->res_capacity) return TGB_OK;
-    if (c->R) cudaFree(c->R);
-    c->R = nullptr; c->res_capacity = 0;
-    for (Wavefront &w : c->wf) w.sr.R = nullptr;
-    CU(cudaMalloc(reinterpret_cast<void **>(&c->R), n_paths*sizeof(float4)));
-    c->res_capacity = n_paths;
-    for (Wavefront &w : c->wf) w.sr.R = c->R;
+    const cudaError_t e = c->R.ensure(n_paths);
+    for (Wavefront &w : c->wf) w.sr.R = c->R.p;               // (null after a failed allocation)
+    CU(e);
     return TGB_OK;
 }
 
@@ -421,7 +468,7 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const Batc
         if (rc) return rc;
         BatchInfo bi;
         if (run) bi = *run;
-        else { bi.pix_id = c->pix_id; bi.pix_seed = c->pix_seed; bi.n_pix = n_pix; bi.pix_first = nullptr; bi.pix_base = nullptr; bi.pix_bits = pix_bits; }
+        else { bi.pix_id = c->pix_id.p; bi.pix_seed = c->pix_seed.p; bi.n_pix = n_pix; bi.pix_first = nullptr; bi.pix_base = nullptr; bi.pix_bits = pix_bits; }
         bi.spp_begin = spp_begin + s0;
         // fork: wavefront 1 starts behind what the caller's stream holds so far (the previous sub-step's k_resolve reads R)
         const cudaStream_t st[2] = {c->stream, c->stream1};
@@ -438,7 +485,7 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const Batc
             const uint32_t base = h ? half : 0, end = h ? total : half;
             if (end == base) continue;
             // control block of the first iteration; from then on k_iter_end keeps it
-            Ctl &init = w.h_ctl[4];
+            Ctl &init = w.h_ctl.p[4];
             std::memset(&init, 0, sizeof(Ctl));
             init.capacity = w.capacity; init.total = end; init.first_path = base;
             init.n_new = std::min(w.capacity, end - base); init.n = init.n_new; init.issued = base + init.n_new;
@@ -456,7 +503,7 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const Batc
                 Wavefront &w = c->wf[h];
                 enqueue_iteration(c, w, st[h], bi, cur[h], bound[h], slot, launches);
                 cur[h] ^= 1;
-                CU(cudaMemcpyAsync(&w.h_ctl[slot], w.ctl, sizeof(Ctl), cudaMemcpyDeviceToHost, st[h]));
+                CU(cudaMemcpyAsync(&w.h_ctl.p[slot], w.ctl, sizeof(Ctl), cudaMemcpyDeviceToHost, st[h]));
                 CU(cudaEventRecord(w.ev_ring[slot], st[h]));
             }
             if (iter == 0) continue;                          // nothing known yet about iteration 1: its bound stays the first one
@@ -465,7 +512,7 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const Batc
                 if (!live[h]) continue;
                 Wavefront &w = c->wf[h];
                 CU(cudaEventSynchronize(w.ev_ring[p]));
-                const Ctl S = w.h_ctl[p];                     // state after iteration iter-1 = the sizes of iteration iter
+                const Ctl S = w.h_ctl.p[p];                   // state after iteration iter-1 = the sizes of iteration iter
                 if (c->profiling) {
                     for (int k = 0; k < 7; ++k) { float ms = 0.0f; cudaEventElapsedTime(&ms, w.ev_k[p][k], w.ev_k[p][k + 1]); kms[k] += ms; }
                     trace_launches++; shadow_launches++;       // one k_trace and one k_shadow_bvh per timed iteration
@@ -480,16 +527,16 @@ int render_device(tgb_ctx *c, uint32_t spp_begin, uint32_t spp_count, const Batc
         // join: k_resolve, and whatever the caller queues on its stream after this call, wait for wavefront 1
         CU(cudaEventRecord(c->ev_join, st[1]));
         CU(cudaStreamWaitEvent(st[0], c->ev_join, 0));
-        k_resolve<<<blocks(n_pix, 256), 256, 0, st[0]>>>(c->R, bi, ns, c->fb, c->fb_count); launches++;
+        k_resolve<<<blocks(n_pix, 256), 256, 0, st[0]>>>(c->R.p, bi, ns, c->fb, c->fb_count); launches++;
     }
     CU(cudaEventRecord(c->ev1, c->stream));
-    CU(cudaMemcpyAsync(c->h_ctr, c->ctr, sizeof(Counters), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(c->h_ctr.p, c->ctr, sizeof(Counters), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     CU(cudaGetLastError());
     float ms = 0.0f; cudaEventElapsedTime(&ms, c->ev0, c->ev1);
     c->stats.samples += samples_done;
-    c->stats.path_rays = c->h_ctr->rays; c->stats.shadow_rays = c->h_ctr->shadow_rays;
-    c->stats.rays = c->h_ctr->rays + c->h_ctr->shadow_rays; c->stats.hits = c->h_ctr->hits + c->h_ctr->shadow_hits;
+    c->stats.path_rays = c->h_ctr.p->rays; c->stats.shadow_rays = c->h_ctr.p->shadow_rays;
+    c->stats.rays = c->h_ctr.p->rays + c->h_ctr.p->shadow_rays; c->stats.hits = c->h_ctr.p->hits + c->h_ctr.p->shadow_hits;
     trace_ms = float(kms[1]); shadow_ms = float(kms[4]);
     c->stats.regen_ms += kms[0]; c->stats.shade_ms += kms[2]; c->stats.prep_ms += kms[3]; c->stats.accum_ms += kms[5]; c->stats.sort_ms += kms[6];
     c->stats.iterations += iterations;
@@ -550,35 +597,28 @@ int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
         for (uint32_t i = 0; i < runs[k].n; ++i) { f[i] = slot; slot += cnt[runs[k].p0 + i]; }
         f[runs[k].n] = slot;
     }
-    if (c->adaptive_capacity < first.size() || !c->rec_dev) {
-        if ((rc = dev_alloc(c, &c->pix_first, first.size()))) return rc;
-        if ((rc = dev_alloc(c, &c->pix_base, first.size()))) return rc;
-        if (!c->pix_slot && (rc = dev_alloc(c, &c->pix_slot, size_t(c->res_x)*c->res_y))) return rc;
-        if (!c->rec_dev && (rc = dev_alloc(c, &c->rec_dev, n_blocks))) return rc;
-        c->adaptive_capacity = uint32_t(first.size());
-    }
     if (!c->pix_slot_valid) {
         std::vector<uint32_t> slot(size_t(c->res_x)*c->res_y, 0xFFFFFFFFu);
         for (uint32_t i = 0; i < c->n_pix; ++i) slot[c->h_pix_id[i]] = i;
-        CU(cudaMemcpyAsync(c->pix_slot, slot.data(), slot.size()*4, cudaMemcpyHostToDevice, c->stream));
+        CU(c->pix_slot.upload(slot.data(), slot.size(), c->stream));
         CU(cudaStreamSynchronize(c->stream));
         c->pix_slot_valid = true;
     }
-    CU(cudaMemcpyAsync(c->pix_first, first.data(), first.size()*4, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->pix_base, base.data(), base.size()*4, cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->rec_dev, records, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyHostToDevice, c->stream));
+    CU(c->pix_first.upload(first.data(), first.size(), c->stream));
+    CU(c->pix_base.upload(base.data(), base.size(), c->stream));
+    CU(c->rec_dev.upload(reinterpret_cast<const SampleRecordD *>(records), n_blocks, c->stream));
     CU(cudaStreamSynchronize(c->stream));                       // (the host vectors go out of scope)
     if (step_total == 0) return TGB_OK;
     for (size_t k = 0; k < runs.size(); ++k) {
         const Run &r = runs[k];
         if (r.total == 0) continue;
-        BatchInfo bi; bi.pix_id = c->pix_id + r.p0; bi.pix_seed = c->pix_seed + r.p0; bi.n_pix = r.n; bi.spp_begin = 0;
-        bi.pix_first = c->pix_first + r.p0 + k; bi.pix_base = c->pix_base + r.p0; bi.pix_bits = index_bits(r.n);
+        BatchInfo bi; bi.pix_id = c->pix_id.p + r.p0; bi.pix_seed = c->pix_seed.p + r.p0; bi.n_pix = r.n; bi.spp_begin = 0;
+        bi.pix_first = c->pix_first.p + r.p0 + k; bi.pix_base = c->pix_base.p + r.p0; bi.pix_bits = index_bits(r.n);
         if ((rc = render_device(c, 0, 0, &bi, uint32_t(r.total)))) return rc;
-        k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R, bi, c->pix_slot, r.p0, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev);
+        k_block_stats<<<blocks(n_blocks, 128), 128, 0, c->stream>>>(c->R.p, bi, c->pix_slot.p, r.p0, c->res_x, c->res_y, var_w, n_blocks, c->rec_dev.p);
         c->stats.kernel_launches++;
     }
-    CU(cudaMemcpyAsync(records, c->rec_dev, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(records, c->rec_dev.p, size_t(n_blocks)*sizeof(SampleRecordD), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     CU(cudaGetLastError());
     return TGB_OK;
@@ -587,7 +627,7 @@ int single_render_adaptive(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, 
 // apply f to every member of a multi-GPU context (the root last, so that the current device ends up being the root's)
 template <class F> int for_members(tgb_ctx *c, F f) {
     if (!c->group) return TGB_OK;
-    Group *g = c->group;
+    Group *g = c->group.get();
     for (size_t k = g->members.size(); k-- > 1;) { int rc = f(g->members[k]); if (rc) { c->error = g->members[k]->error; return rc; } }
     return TGB_OK;
 }
@@ -608,6 +648,7 @@ int group_deal(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_t 
     tgb_ctx *c = root; Group &g = *root->group;
     std::vector<tgb_tile> list = call_tiles(root, tiles, n_tiles, seed);
     if (same_tiles(list, g.deal_key)) return TGB_OK;
+    g.deal_key.clear();                                         // (until the new deal is complete)
     std::vector<uint32_t> pid;
     if (int rc = tile_pixels(root, list, pid)) return rc;     // the whole list: no pixel is rendered by two members
     const size_t N = g.members.size();
@@ -615,34 +656,22 @@ int group_deal(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_t 
     g.shares.assign(N, {});
     for (uint32_t i = 0; i < list.size(); ++i) g.shares[i % N].push_back(list[order[i]]);
     CU(cudaSetDevice(root->device));
-    for (uint32_t *p : g.root_pix) if (p) cudaFree(p);
-    g.root_pix.assign(N, nullptr); g.share_pixels.assign(N, 0);
+    g.root_pix.resize(N); g.share_pixels.assign(N, 0);
     size_t max_share = 0;
     for (size_t k = 0; k < N; ++k) {
         if (int rc = tile_pixels(root, g.shares[k], pid)) return rc;
         g.share_pixels[k] = uint32_t(pid.size());
         max_share = std::max(max_share, pid.size());
-        if (k >= 1 && !pid.empty()) {
-            CU(cudaMalloc(reinterpret_cast<void **>(&g.root_pix[k]), pid.size()*4));
-            CU(cudaMemcpy(g.root_pix[k], pid.data(), pid.size()*4, cudaMemcpyHostToDevice));
+        if (k >= 1) {
+            CU(g.root_pix[k].upload(pid.data(), pid.size(), root->stream));
+            CU(cudaStreamSynchronize(root->stream));
         }
     }
-    if (max_share > g.recv_capacity) {
-        if (g.recv) cudaFree(g.recv);
-        g.recv = nullptr; g.recv_capacity = 0;
-        CU(cudaMalloc(reinterpret_cast<void **>(&g.recv), max_share*sizeof(float4)));
-        g.recv_capacity = max_share;
-    }
-    g.send.resize(N, nullptr); g.send_capacity.resize(N, 0);
+    CU(g.recv.ensure(max_share));
     for (size_t k = 1; k < N; ++k) {
-        if (g.share_pixels[k] > g.send_capacity[k]) {
-            tgb_ctx *m = g.members[k];
-            if (cudaSetDevice(m->device) != cudaSuccess) return fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", m->device);
-            if (g.send[k]) cudaFree(g.send[k]);
-            g.send[k] = nullptr; g.send_capacity[k] = 0;
-            if (cudaMalloc(reinterpret_cast<void **>(&g.send[k]), size_t(g.share_pixels[k])*sizeof(float4)) != cudaSuccess) return fail(c, TGB_ERR_OOM, "gather buffer allocation failed on device %d", m->device);
-            g.send_capacity[k] = g.share_pixels[k];
-        }
+        tgb_ctx *m = g.members[k];
+        if (cudaSetDevice(m->device) != cudaSuccess) return fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", m->device);
+        CU(m->send.ensure(g.share_pixels[k]));
     }
     g.deal_key = std::move(list);
     return TGB_OK;
@@ -678,28 +707,25 @@ int group_render(tgb_ctx *root, const tgb_tile *tiles, uint32_t n_tiles, uint32_
     }
     // gather: pack on the member, one peer copy, de-tile on the root
     CU(cudaSetDevice(root->device));
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    CU(cudaEventCreate(&e0)); CU(cudaEventCreate(&e1));
-    CU(cudaEventRecord(e0, root->stream));
+    CU(cudaEventRecord(g.ev_gather[0], root->stream));
     for (size_t k = 1; k < N; ++k) {
         tgb_ctx *m = g.members[k];
         const uint32_t np = g.share_pixels[k];
         if (!np) continue;
         if (cudaSetDevice(m->device) != cudaSuccess) return fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", m->device);
-        k_pack_share<<<blocks(np, 256), 256, 0, m->stream>>>(m->pix_id, np, m->fb, m->fb_count, g.send[k]);
+        k_pack_share<<<blocks(np, 256), 256, 0, m->stream>>>(m->pix_id.p, np, m->fb, m->fb_count, m->send.p);
         m->stats.kernel_launches++;
         cudaError_t e = cudaStreamSynchronize(m->stream);
         if (e != cudaSuccess) return fail(c, TGB_ERR_CUDA, "pack on device %d failed: %s", m->device, cudaGetErrorString(e));
         CU(cudaSetDevice(root->device));
-        CU(cudaMemcpyPeerAsync(g.recv, root->device, g.send[k], m->device, size_t(np)*sizeof(float4), root->stream));
-        k_unpack_share<<<blocks(np, 256), 256, 0, root->stream>>>(g.root_pix[k], np, g.recv, root->fb, root->fb_count);
+        CU(cudaMemcpyPeerAsync(g.recv.p, root->device, m->send.p, m->device, size_t(np)*sizeof(float4), root->stream));
+        k_unpack_share<<<blocks(np, 256), 256, 0, root->stream>>>(g.root_pix[k].p, np, g.recv.p, root->fb, root->fb_count);
         root->stats.kernel_launches++;
     }
     CU(cudaSetDevice(root->device));
-    CU(cudaEventRecord(e1, root->stream));
+    CU(cudaEventRecord(g.ev_gather[1], root->stream));
     CU(cudaStreamSynchronize(root->stream));
-    float ms = 0.0f; cudaEventElapsedTime(&ms, e0, e1); g.gather_ms += ms;
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    float ms = 0.0f; cudaEventElapsedTime(&ms, g.ev_gather[0], g.ev_gather[1]); g.gather_ms += ms;
     CU(cudaGetLastError());
     return TGB_OK;
 }
@@ -718,7 +744,6 @@ int check_settings(const tgb_scene_desc *d) {
 
 // A context for a prepared scene on device dev (< 0: the current device)
 int create_single(const HostScene &hs, int dev, tgb_ctx **out) {
-    tgb_ctx *c = nullptr;
     *out = nullptr;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(nullptr, TGB_ERR_NO_DEVICE, "no CUDA device available (this library has no CPU fallback)"); }
@@ -727,21 +752,11 @@ int create_single(const HostScene &hs, int dev, tgb_ctx **out) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, dev) != cudaSuccess) return fail(nullptr, TGB_ERR_NO_DEVICE, "cannot query device %d", dev);
     if (prop.major != 9 || prop.minor != 0) return fail(nullptr, TGB_ERR_NO_DEVICE, "device %d is sm_%d%d; this library is built for sm_90a only", dev, prop.major, prop.minor);
-    c = new tgb_ctx();
-    c->device = dev;
+    if (cudaSetDevice(dev) != cudaSuccess) return fail(nullptr, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", dev);
+    tgb_ctx *c = new tgb_ctx(dev);
     int rc = TGB_OK;
     do {
-        if (cudaSetDevice(dev) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaSetDevice(%d) failed", dev); break; }
-        if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
-            cudaStreamCreateWithFlags(&c->stream1, cudaStreamNonBlocking) != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "cudaStreamCreate failed"); break; }
-        c->stream = c->own_stream;
-        for (cudaEvent_t *e : {&c->ev0, &c->ev1}) cudaEventCreate(e);
-        for (cudaEvent_t *e : {&c->ev_fork, &c->ev_join}) cudaEventCreateWithFlags(e, cudaEventDisableTiming);
-        for (Wavefront &w : c->wf)
-            for (int k = 0; k < 4; ++k) {
-                cudaEventCreateWithFlags(&w.ev_ring[k], cudaEventDisableTiming);
-                for (cudaEvent_t &e : w.ev_k[k]) cudaEventCreate(&e);
-            }
+        if (c->created != cudaSuccess) { rc = fail(c, TGB_ERR_CUDA, "stream or event creation failed: %s", cudaGetErrorString(c->created)); break; }
         c->ks = select_kernels(hs.kind);
         if ((rc = upload_scene(c, hs, c->ks))) break;
         // default: 2 x 4 Mi paths in flight (H100, C1: 2 x 2 Mi measured 3 % slower)
@@ -780,16 +795,15 @@ int create_single(const HostScene &hs, int dev, tgb_ctx **out) {
 
 // Closest hits of n device rays through the analytic pass and the renderer's traversal kernels (into device Hit records)
 // As in a render, rays that miss the BVH's top-level cut before their analytic hit skip the traversal (TGB_HOOK_CUT=0: every ray
-// is traversed).
-cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t n) {
+// is traversed).  list: the traversal list, [count | indices of the rays to traverse], which the caller keeps until its stream
+// has run the kernels.
+cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t n, Buffer<uint32_t> &list) {
     const char *cut_env = getenv("TGB_HOOK_CUT");
     const int cut = (cut_env && cut_env[0] == '0') ? 0 : 1;
-    uint32_t *list = nullptr;                                   // [count | indices of the rays to traverse]
-    cudaError_t e = cudaMallocAsync(reinterpret_cast<void **>(&list), (size_t(n) + 1)*sizeof(uint32_t), c->stream);
-    if (e != cudaSuccess) return e;
-    e = cudaMemsetAsync(list, 0, sizeof(uint32_t), c->stream);
+    cudaError_t e = list.ensure(size_t(n) + 1);
+    if (e == cudaSuccess) e = cudaMemsetAsync(list.p, 0, sizeof(uint32_t), c->stream);
     if (e == cudaSuccess) {
-        k_hook_analytic<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, n, cut, list + 1, list);
+        k_hook_analytic<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, n, cut, list.p + 1, list.p);
         c->stats.kernel_launches++;
     }
     if (e == cudaSuccess && c->sc.n_nodes) {
@@ -797,29 +811,22 @@ cudaError_t hook_closest(tgb_ctx *c, const tgb_ray *dr, Hit *dx, uint32_t n) {
         uint32_t *cursor = &c->wf[0].ctl->cursor_trace;
         e = cudaMemsetAsync(cursor, 0, sizeof(uint32_t), c->stream);
         uint32_t grid = std::min(blocks(n, kTraceBlock), c->persist_blocks);
-        if (e == cudaSuccess) c->ks.hook_persist<<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list + 1, list, n, cursor);
+        if (e == cudaSuccess) c->ks.hook_persist<<<grid, kTraceBlock, 0, c->stream>>>(c->sc, dr, dx, list.p + 1, list.p, n, cursor);
         c->stats.kernel_launches++;
     }
-    const cudaError_t ef = cudaFreeAsync(list, c->stream);
-    return e != cudaSuccess ? e : ef;
+    return e;
 }
 
-// the pixel list of tgb200_pack_tiles / tgb200_unpack_tiles on the device (owned: a copy the caller frees)
-int device_tile_pixels(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uint32_t **dev, uint32_t *n_out, bool *owned) {
-    *owned = true;
+// The pixel list of tgb200_pack_tiles / tgb200_unpack_tiles on the device: the last render's when the tile list is the same,
+// else a copy in `own`
+int device_tile_pixels(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, Buffer<uint32_t> &own, const uint32_t **dev, uint32_t *n_out) {
     const std::vector<tgb_tile> list(tiles, tiles + n_tiles);
-    if (same_tiles(list, c->tiles_cached)) {
-        *dev = c->pix_id; *n_out = c->n_pix; *owned = false;      // same tile list as the last render: reuse its pixel list
-        return TGB_OK;
-    }
+    if (same_tiles(list, c->tiles_cached)) { *dev = c->pix_id.p; *n_out = c->n_pix; return TGB_OK; }
     std::vector<uint32_t> pid;
     if (int rc = tile_pixels(c, list, pid)) return rc;
-    *n_out = uint32_t(pid.size()); *dev = nullptr;
-    if (pid.empty()) return TGB_OK;
-    CU(cudaMalloc(reinterpret_cast<void **>(dev), pid.size()*4));
-    cudaError_t e = cudaMemcpyAsync(*dev, pid.data(), pid.size()*4, cudaMemcpyHostToDevice, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) { cudaFree(*dev); *dev = nullptr; return fail(c, TGB_ERR_CUDA, "tile upload failed: %s", cudaGetErrorString(e)); }
+    CU(own.upload(pid.data(), pid.size(), c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    *dev = own.p; *n_out = uint32_t(pid.size());
     return TGB_OK;
 }
 
@@ -863,39 +870,26 @@ bool host_triangle(const IsectRecord &rec, const V3 &o, const V3 &d, float tnear
 }
 
 // ---- test hooks: host arrays in, one probe kernel on the context's stream, host arrays out ----
-struct ProbeBufs {                  // device copies of a probe's arrays, freed on every exit
-    tgb_ctx *c; std::vector<void *> p;
-    Ctl *ctl_saved = nullptr; Counters *ctr_saved = nullptr; bool saved = false;
+// A probe's end: the restore of the state it saved, then the synchronise after which its arrays (Buffers declared in the probe)
+// may be freed
+struct ProbeBufs {
+    tgb_ctx *c;
+    Buffer<Ctl> ctl_saved; Buffer<Counters> ctr_saved; bool saved = false;
     explicit ProbeBufs(tgb_ctx *ctx) : c(ctx) {}
-    ~ProbeBufs() { for (void *q : p) cudaFree(q); }
-    template <typename T> cudaError_t alloc(T **out, size_t n) {
-        void *q = nullptr;
-        cudaError_t e = cudaMalloc(&q, std::max<size_t>(n, 1)*sizeof(T));
-        if (e == cudaSuccess) p.push_back(q);
-        *out = static_cast<T *>(q);
-        return e;
-    }
-    template <typename T> cudaError_t upload(T **out, const T *src, size_t n) {
-        cudaError_t e = alloc(out, n);
-        return e != cudaSuccess ? e : cudaMemcpyAsync(*out, src, n*sizeof(T), cudaMemcpyHostToDevice, c->stream);
-    }
-    template <typename T> cudaError_t download(T *dst, const T *src, size_t n) {
-        return cudaMemcpyAsync(dst, src, n*sizeof(T), cudaMemcpyDeviceToHost, c->stream);
-    }
     // Snapshot of wavefront 0's control block and the context's counters, which a probe that runs the renderer's kernels uses:
     // its launches must not show in them or in the next render's statistics.  finish() queues the restore.
     cudaError_t save_state() {
-        cudaError_t e = alloc(&ctl_saved, 1);
-        if (e == cudaSuccess) e = alloc(&ctr_saved, 1);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved, c->wf[0].ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
+        cudaError_t e = ctl_saved.ensure(1);
+        if (e == cudaSuccess) e = ctr_saved.ensure(1);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctl_saved.p, c->wf[0].ctl, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(ctr_saved.p, c->ctr, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
         saved = e == cudaSuccess;
         return e;
     }
     int finish(cudaError_t e, const char *what) {
         if (saved) {        // also when a launch failed: the copies are queued after whatever was queued
-            const cudaError_t r1 = cudaMemcpyAsync(c->wf[0].ctl, ctl_saved, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
-            const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
+            const cudaError_t r1 = cudaMemcpyAsync(c->wf[0].ctl, ctl_saved.p, sizeof(Ctl), cudaMemcpyDeviceToDevice, c->stream);
+            const cudaError_t r2 = cudaMemcpyAsync(c->ctr, ctr_saved.p, sizeof(Counters), cudaMemcpyDeviceToDevice, c->stream);
             if (e == cudaSuccess) e = r1 != cudaSuccess ? r1 : r2;
         }
         if (e == cudaSuccess) e = cudaGetLastError();
@@ -903,6 +897,9 @@ struct ProbeBufs {                  // device copies of a probe's arrays, freed 
         return e == cudaSuccess ? TGB_OK : fail(c, TGB_ERR_CUDA, "%s failed: %s", what, cudaGetErrorString(e));
     }
 };
+template <typename T> cudaError_t download(tgb_ctx *c, T *dst, const T *src, size_t n) {
+    return cudaMemcpyAsync(dst, src, n*sizeof(T), cudaMemcpyDeviceToHost, c->stream);
+}
 // lobe_set 1 (the Lambert-only instantiation) exists only without curves, as in k_shade
 int probe_check(tgb_ctx *c, int lobe_set) {
     if (lobe_set != 0 && lobe_set != 1) return fail(c, TGB_ERR_INVALID, "lobe_set must be 0 or 1");
@@ -919,34 +916,11 @@ const char *tgb200_last_error(const tgb_ctx *ctx) { return ctx ? ctx->error.c_st
 
 void tgb200_destroy(tgb_ctx *c) {
     if (!c) return;
-    if (c->group) {
-        Group *g = c->group; c->group = nullptr;
-        cudaSetDevice(c->device);
-        for (uint32_t *p : g->root_pix) if (p) cudaFree(p);
-        if (g->recv) cudaFree(g->recv);
-        for (size_t k = 1; k < g->members.size(); ++k) {
-            cudaSetDevice(g->members[k]->device);
-            if (k < g->send.size() && g->send[k]) cudaFree(g->send[k]);
-            tgb200_destroy(g->members[k]);
-        }
-        delete g;
-    }
+    if (c->group) for (size_t k = 1; k < c->group->members.size(); ++k) tgb200_destroy(c->group->members[k]);
     cudaSetDevice(c->device);
     if (c->stream) cudaStreamSynchronize(c->stream);
     if (c->stream1) cudaStreamSynchronize(c->stream1);
-    for (void *p : c->allocs) cudaFree(p);
-    if (c->R) cudaFree(c->R);
-    if (c->h_ctr) cudaFreeHost(c->h_ctr);
-    if (c->h_fb) cudaFreeHost(c->h_fb);
-    if (c->h_fb_count) cudaFreeHost(c->h_fb_count);
-    for (cudaEvent_t e : {c->ev0, c->ev1, c->ev_fork, c->ev_join}) if (e) cudaEventDestroy(e);
-    for (Wavefront &w : c->wf) {
-        if (w.h_ctl) cudaFreeHost(w.h_ctl);
-        for (int k = 0; k < 4; ++k) { if (w.ev_ring[k]) cudaEventDestroy(w.ev_ring[k]); for (cudaEvent_t e : w.ev_k[k]) if (e) cudaEventDestroy(e); }
-    }
-    if (c->stream1) cudaStreamDestroy(c->stream1);
-    if (c->own_stream) cudaStreamDestroy(c->own_stream);
-    delete c;
+    delete c;               // with its group, which lives on this device
 }
 
 int tgb200_create(const tgb_scene_desc *d, tgb_ctx **out) {
@@ -981,8 +955,11 @@ int tgb200_create(const tgb_scene_desc *d, tgb_ctx **out) {
         cudaGetLastError();
     }
     cudaSetDevice(root->device);
-    root->group = new Group();
-    root->group->members = members;
+    root->group = std::make_unique<Group>(members);
+    if (const cudaError_t e = root->group->created; e != cudaSuccess) {
+        tgb200_destroy(root);
+        return fail(nullptr, TGB_ERR_CUDA, "cudaEventCreate failed: %s", cudaGetErrorString(e));
+    }
     *out = root;
     return TGB_OK;
 }
@@ -1009,11 +986,11 @@ int tgb200_read_framebuffer(tgb_ctx *c, float *rgb_mean, uint32_t *count) {
     if (!c || !rgb_mean) return TGB_ERR_INVALID;
     CU(cudaSetDevice(c->device));
     size_t npx = size_t(c->res_x)*c->res_y;
-    CU(cudaMemcpyAsync(c->h_fb, c->fb, npx*3*sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    if (count) CU(cudaMemcpyAsync(c->h_fb_count, c->fb_count, npx*sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(c->h_fb.p, c->fb, npx*3*sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    if (count) CU(cudaMemcpyAsync(c->h_fb_count.p, c->fb_count, npx*sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
-    std::memcpy(rgb_mean, c->h_fb, npx*3*sizeof(float));
-    if (count) std::memcpy(count, c->h_fb_count, npx*sizeof(uint32_t));
+    std::memcpy(rgb_mean, c->h_fb.p, npx*3*sizeof(float));
+    if (count) std::memcpy(count, c->h_fb_count.p, npx*sizeof(uint32_t));
     return TGB_OK;
 }
 
@@ -1021,31 +998,13 @@ int tgb200_render_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, uin
                         float *rgb_mean, uint32_t *count) {
     if (!c || !rgb_mean) return c ? fail(c, TGB_ERR_INVALID, "null framebuffer") : TGB_ERR_INVALID;
     if (n_tiles && !tiles) return fail(c, TGB_ERR_INVALID, "null tile list");
-    if (c->group) {         // every member needs the caller's running means for its own pixels
-        std::vector<uint32_t> base;
-        if (!count) base.assign(size_t(c->res_x)*c->res_y, spp_begin);
-        int rc = tgb200_write_framebuffer(c, rgb_mean, count ? count : base.data());
-        if (rc) return rc;
-        if ((rc = group_render(c, tiles, n_tiles, seed, spp_begin, spp_count, nullptr))) return rc;
-        return tgb200_read_framebuffer(c, rgb_mean, count);
-    }
-    CU(cudaSetDevice(c->device));
-    size_t npx = size_t(c->res_x)*c->res_y;
-    // host -> device: the caller's running mean and counts are the input state
-    std::memcpy(c->h_fb, rgb_mean, npx*3*sizeof(float));
-    CU(cudaMemcpyAsync(c->fb, c->h_fb, npx*3*sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    if (count) {
-        std::memcpy(c->h_fb_count, count, npx*sizeof(uint32_t));
-        CU(cudaMemcpyAsync(c->fb_count, c->h_fb_count, npx*sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    } else {
-        // without counts the running mean restarts from the sample index range's start
-        std::vector<uint32_t> base(npx, spp_begin);
-        std::memcpy(c->h_fb_count, base.data(), npx*sizeof(uint32_t));
-        CU(cudaMemcpyAsync(c->fb_count, c->h_fb_count, npx*sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    }
-    int rc = set_tiles(c, tiles, n_tiles, seed);
+    // the caller's running mean and counts are the input state (of every member of a multi-GPU context, for its own pixels);
+    // without counts the running mean restarts from the sample index range's start
+    std::vector<uint32_t> base;
+    if (!count) base.assign(size_t(c->res_x)*c->res_y, spp_begin);
+    int rc = tgb200_write_framebuffer(c, rgb_mean, count ? count : base.data());
     if (rc) return rc;
-    if ((rc = render_device(c, spp_begin, spp_count))) return rc;
+    if ((rc = tgb200_render_resident(c, tiles, n_tiles, seed, spp_begin, spp_count))) return rc;
     return tgb200_read_framebuffer(c, rgb_mean, count);
 }
 
@@ -1060,24 +1019,18 @@ int tgb200_trace_closest(tgb_ctx *c, const tgb_ray *rays, tgb_hit *hits, uint32_
     if (!c || (n && (!rays || !hits))) return TGB_ERR_INVALID;
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
-    tgb_ray *dr = nullptr; tgb_hit *dh = nullptr; Hit *dx = nullptr;
-    CU(cudaMalloc(reinterpret_cast<void **>(&dr), size_t(n)*sizeof(tgb_ray)));
-    cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&dh), size_t(n)*sizeof(tgb_hit));
-    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void **>(&dx), size_t(n)*sizeof(Hit));
-    if (e != cudaSuccess) { cudaFree(dr); cudaFree(dh); return fail(c, TGB_ERR_OOM, "cudaMalloc failed: %s", cudaGetErrorString(e)); }
-    int rc = TGB_OK;
-    do {
-        if ((e = cudaMemcpyAsync(dr, rays, size_t(n)*sizeof(tgb_ray), cudaMemcpyHostToDevice, c->stream)) != cudaSuccess) break;
-        if ((e = hook_closest(c, dr, dx, n)) != cudaSuccess) break;
-        k_hook_finish<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr, dx, dh, n);
+    Buffer<tgb_ray> dr; Buffer<tgb_hit> dh; Buffer<Hit> dx; Buffer<uint32_t> list;
+    CU(dr.ensure(n)); CU(dh.ensure(n)); CU(dx.ensure(n));
+    cudaError_t e = cudaMemcpyAsync(dr.p, rays, size_t(n)*sizeof(tgb_ray), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = hook_closest(c, dr.p, dx.p, n, list);
+    if (e == cudaSuccess) {
+        k_hook_finish<<<blocks(n, 256), 256, 0, c->stream>>>(c->sc, dr.p, dx.p, dh.p, n);
         c->stats.kernel_launches++;
-        if ((e = cudaMemcpyAsync(hits, dh, size_t(n)*sizeof(tgb_hit), cudaMemcpyDeviceToHost, c->stream)) != cudaSuccess) break;
-        e = cudaStreamSynchronize(c->stream);
-        if (e == cudaSuccess) e = cudaGetLastError();
-    } while (0);
-    if (e != cudaSuccess) rc = fail(c, TGB_ERR_CUDA, "trace_closest failed: %s", cudaGetErrorString(e));
-    cudaFree(dr); cudaFree(dh); cudaFree(dx);
-    return rc;
+        e = cudaMemcpyAsync(hits, dh.p, size_t(n)*sizeof(tgb_hit), cudaMemcpyDeviceToHost, c->stream);
+    }
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (e == cudaSuccess) e = cudaGetLastError();
+    return e == cudaSuccess ? TGB_OK : fail(c, TGB_ERR_CUDA, "trace_closest failed: %s", cudaGetErrorString(e));
 }
 
 int tgb200_get_stats(tgb_ctx *c, tgb_stats *out) {
@@ -1139,13 +1092,12 @@ int tgb200_scene_info(tgb_ctx *c, uint32_t *n_tris, uint32_t *n_nodes, uint32_t 
 int tgb200_pack_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, void *rgb_out_dev) {
     if (!c || !tiles || !rgb_out_dev) return TGB_ERR_INVALID;
     CU(cudaSetDevice(c->device));
-    uint32_t *pid = nullptr, n = 0; bool owned = true;
-    int rc = device_tile_pixels(c, tiles, n_tiles, &pid, &n, &owned);
+    Buffer<uint32_t> own; const uint32_t *pid = nullptr; uint32_t n = 0;
+    int rc = device_tile_pixels(c, tiles, n_tiles, own, &pid, &n);
     if (rc || !n) return rc;
     k_pack_tiles<<<blocks(n, 256), 256, 0, c->stream>>>(pid, n, c->fb, static_cast<float *>(rgb_out_dev));
     c->stats.kernel_launches++;
     cudaError_t e = cudaStreamSynchronize(c->stream);
-    if (owned) cudaFree(pid);
     if (e != cudaSuccess) return fail(c, TGB_ERR_CUDA, "pack_tiles failed: %s", cudaGetErrorString(e));
     return TGB_OK;
 }
@@ -1153,13 +1105,12 @@ int tgb200_pack_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, void 
 int tgb200_unpack_tiles(tgb_ctx *c, const tgb_tile *tiles, uint32_t n_tiles, const void *rgb_in_dev, uint32_t sample_count) {
     if (!c || !tiles || !rgb_in_dev) return TGB_ERR_INVALID;
     CU(cudaSetDevice(c->device));
-    uint32_t *pid = nullptr, n = 0; bool owned = true;
-    int rc = device_tile_pixels(c, tiles, n_tiles, &pid, &n, &owned);
+    Buffer<uint32_t> own; const uint32_t *pid = nullptr; uint32_t n = 0;
+    int rc = device_tile_pixels(c, tiles, n_tiles, own, &pid, &n);
     if (rc || !n) return rc;
     k_unpack_tiles<<<blocks(n, 256), 256, 0, c->stream>>>(pid, n, static_cast<const float *>(rgb_in_dev), c->fb, c->fb_count, sample_count);
     c->stats.kernel_launches++;
     cudaError_t e = cudaStreamSynchronize(c->stream);
-    if (owned) cudaFree(pid);
     if (e != cudaSuccess) return fail(c, TGB_ERR_CUDA, "unpack_tiles failed: %s", cudaGetErrorString(e));
     return TGB_OK;
 }
@@ -1230,9 +1181,9 @@ int tgb200_write_framebuffer(tgb_ctx *c, const float *rgb_mean, const uint32_t *
     { int rc = for_members(c, [=](tgb_ctx *m) { return tgb200_write_framebuffer(m, rgb_mean, count); }); if (rc) return rc; }
     CU(cudaSetDevice(c->device));
     size_t npx = size_t(c->res_x)*c->res_y;
-    std::memcpy(c->h_fb, rgb_mean, npx*3*sizeof(float)); std::memcpy(c->h_fb_count, count, npx*sizeof(uint32_t));
-    CU(cudaMemcpyAsync(c->fb, c->h_fb, npx*3*sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    CU(cudaMemcpyAsync(c->fb_count, c->h_fb_count, npx*sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    std::memcpy(c->h_fb.p, rgb_mean, npx*3*sizeof(float)); std::memcpy(c->h_fb_count.p, count, npx*sizeof(uint32_t));
+    CU(cudaMemcpyAsync(c->fb, c->h_fb.p, npx*3*sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(c->fb_count, c->h_fb_count.p, npx*sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return TGB_OK;
 }
@@ -1451,15 +1402,15 @@ int tgb200_bsdf_probe(tgb_ctx *c, int bsdf, float u, float v, uint32_t requested
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    float *dw = nullptr, *dout = nullptr;
-    cudaError_t e = b.upload(&dw, wi_wo, 6*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dout, 4*size_t(n));
+    Buffer<float> dw, dout;
+    cudaError_t e = dw.upload(wi_wo, 6*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dout.ensure(4*size_t(n));
     if (e == cudaSuccess) {
         const uint32_t g = blocks(n, 128);
-        if (c->has_curves) k_probe_bsdf<true, 0><<<g, 128, 0, c->stream>>>(c->sc, bsdf, u, v, requested, dw, dout, n);
-        else if (lobe_set == 1) k_probe_bsdf<false, 1><<<g, 128, 0, c->stream>>>(c->sc, bsdf, u, v, requested, dw, dout, n);
-        else k_probe_bsdf<false, 0><<<g, 128, 0, c->stream>>>(c->sc, bsdf, u, v, requested, dw, dout, n);
-        e = b.download(out, dout, 4*size_t(n));
+        if (c->has_curves) k_probe_bsdf<true, 0><<<g, 128, 0, c->stream>>>(c->sc, bsdf, u, v, requested, dw.p, dout.p, n);
+        else if (lobe_set == 1) k_probe_bsdf<false, 1><<<g, 128, 0, c->stream>>>(c->sc, bsdf, u, v, requested, dw.p, dout.p, n);
+        else k_probe_bsdf<false, 0><<<g, 128, 0, c->stream>>>(c->sc, bsdf, u, v, requested, dw.p, dout.p, n);
+        e = download(c, out, dout.p, 4*size_t(n));
     }
     return b.finish(e, "bsdf_probe");
 }
@@ -1473,19 +1424,19 @@ int tgb200_bsdf_sample_probe(tgb_ctx *c, uint32_t seed, uint32_t n, const int *b
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    int *db = nullptr; uint32_t *dpix = nullptr, *dl = nullptr; float *dwi = nullptr, *dout = nullptr;
-    cudaError_t e = b.upload(&db, bsdf, n);
-    if (e == cudaSuccess) e = b.upload(&dpix, pixel_id, n);
-    if (e == cudaSuccess) e = b.upload(&dwi, wi, 3*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dout, 8*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dl, n);
+    Buffer<int> db; Buffer<uint32_t> dpix, dl; Buffer<float> dwi, dout;
+    cudaError_t e = db.upload(bsdf, n, c->stream);
+    if (e == cudaSuccess) e = dpix.upload(pixel_id, n, c->stream);
+    if (e == cudaSuccess) e = dwi.upload(wi, 3*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dout.ensure(8*size_t(n));
+    if (e == cudaSuccess) e = dl.ensure(n);
     if (e == cudaSuccess) {
         const uint32_t g = blocks(n, 128);
-        if (c->has_curves) k_probe_bsdf_sample<true, 0><<<g, 128, 0, c->stream>>>(c->sc, seed, db, dpix, sample, u, v, requested, dwi, dout, dl, n);
-        else if (lobe_set == 1) k_probe_bsdf_sample<false, 1><<<g, 128, 0, c->stream>>>(c->sc, seed, db, dpix, sample, u, v, requested, dwi, dout, dl, n);
-        else k_probe_bsdf_sample<false, 0><<<g, 128, 0, c->stream>>>(c->sc, seed, db, dpix, sample, u, v, requested, dwi, dout, dl, n);
-        e = b.download(out, dout, 8*size_t(n));
-        if (e == cudaSuccess) e = b.download(lobes, dl, n);
+        if (c->has_curves) k_probe_bsdf_sample<true, 0><<<g, 128, 0, c->stream>>>(c->sc, seed, db.p, dpix.p, sample, u, v, requested, dwi.p, dout.p, dl.p, n);
+        else if (lobe_set == 1) k_probe_bsdf_sample<false, 1><<<g, 128, 0, c->stream>>>(c->sc, seed, db.p, dpix.p, sample, u, v, requested, dwi.p, dout.p, dl.p, n);
+        else k_probe_bsdf_sample<false, 0><<<g, 128, 0, c->stream>>>(c->sc, seed, db.p, dpix.p, sample, u, v, requested, dwi.p, dout.p, dl.p, n);
+        e = download(c, out, dout.p, 8*size_t(n));
+        if (e == cudaSuccess) e = download(c, lobes, dl.p, n);
     }
     return b.finish(e, "bsdf_sample_probe");
 }
@@ -1496,16 +1447,16 @@ int tgb200_light_probe(tgb_ctx *c, int prim, uint32_t seed, uint32_t n, uint32_t
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    float *dp = nullptr, *dout = nullptr; tgb_ray *dr = nullptr; Hit *dx = nullptr;
-    cudaError_t e = b.upload(&dp, p, 3*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dout, 12*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dr, n);
-    if (e == cudaSuccess) e = b.alloc(&dx, n);
+    Buffer<float> dp, dout; Buffer<tgb_ray> dr; Buffer<Hit> dx; Buffer<uint32_t> list;
+    cudaError_t e = dp.upload(p, 3*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dout.ensure(12*size_t(n));
+    if (e == cudaSuccess) e = dr.ensure(n);
+    if (e == cudaSuccess) e = dx.ensure(n);
     if (e == cudaSuccess) {
-        k_probe_light<<<blocks(n, 128), 128, 0, c->stream>>>(c->sc, prim, seed, sample, dp, dout, dr, n);
-        if (c->prim_types[size_t(prim)] == TGB_PRIM_MESH &&(e = hook_closest(c, dr, dx, n)) == cudaSuccess)
-            k_probe_light_mesh<<<blocks(n, 128), 128, 0, c->stream>>>(c->sc, prim, dr, dx, dout, n);
-        if (e == cudaSuccess) e = b.download(out, dout, 12*size_t(n));
+        k_probe_light<<<blocks(n, 128), 128, 0, c->stream>>>(c->sc, prim, seed, sample, dp.p, dout.p, dr.p, n);
+        if (c->prim_types[size_t(prim)] == TGB_PRIM_MESH && (e = hook_closest(c, dr.p, dx.p, n, list)) == cudaSuccess)
+            k_probe_light_mesh<<<blocks(n, 128), 128, 0, c->stream>>>(c->sc, prim, dr.p, dx.p, dout.p, n);
+        if (e == cudaSuccess) e = download(c, out, dout.p, 12*size_t(n));
     }
     return b.finish(e, "light_probe");
 }
@@ -1516,13 +1467,13 @@ int tgb200_choose_light_probe(tgb_ctx *c, uint32_t seed, uint32_t n, const uint3
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    uint32_t *dpix = nullptr; float *dp = nullptr, *dout = nullptr;
-    cudaError_t e = b.upload(&dpix, pixel_id, n);
-    if (e == cudaSuccess) e = b.upload(&dp, p, 3*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dout, 2*size_t(n));
+    Buffer<uint32_t> dpix; Buffer<float> dp, dout;
+    cudaError_t e = dpix.upload(pixel_id, n, c->stream);
+    if (e == cudaSuccess) e = dp.upload(p, 3*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dout.ensure(2*size_t(n));
     if (e == cudaSuccess) {
-        k_probe_choose_light<<<blocks(n, 128), 128, 0, c->stream>>>(c->sc, seed, dpix, sample, dp, dout, n);
-        e = b.download(out, dout, 2*size_t(n));
+        k_probe_choose_light<<<blocks(n, 128), 128, 0, c->stream>>>(c->sc, seed, dpix.p, sample, dp.p, dout.p, n);
+        e = download(c, out, dout.p, 2*size_t(n));
     }
     return b.finish(e, "choose_light_probe");
 }
@@ -1535,10 +1486,10 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
     if (n == 0) return TGB_OK;
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    float *dq = nullptr, *dout = nullptr; int *dl = nullptr;
-    cudaError_t e = b.upload(&dq, query, 8*size_t(n));
-    if (e == cudaSuccess) e = b.upload(&dl, light_mis, 2*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dout, 8*size_t(n));
+    Buffer<float> dq, dout; Buffer<int> dl;
+    cudaError_t e = dq.upload(query, 8*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dl.upload(light_mis, 2*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dout.ensure(8*size_t(n));
     if (e == cudaSuccess) e = b.save_state();
     const Wavefront &w = c->wf[0];
     const DScene &sc = c->sc; cudaStream_t st = c->stream;
@@ -1548,16 +1499,16 @@ int tgb200_shadow_probe(tgb_ctx *c, uint32_t n, const float *query, const int *l
         // shadow_count, shadow_count2, cursor_trace, cursor_shadow, shadow_count_closest, cursor_closest
         e = cudaMemsetAsync(&w.ctl->shadow_count, 0, 6*sizeof(uint32_t), st);
         if (e != cudaSuccess) break;
-        k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, w.sr, dq + 8*size_t(off), dl + 2*size_t(off), dout + 8*size_t(off),
+        k_probe_shadow_setup<<<blocks(m, 128), 128, 0, st>>>(sc, w.sr, dq.p + 8*size_t(off), dl.p + 2*size_t(off), dout.p + 8*size_t(off),
                                                             w.squeue, w.ctl, m);
         c->ks.shadow_prep<<<loop_grid(c->prep_blocks, m), 256, 0, st>>>(sc, w.sr, w.squeue, w.ctl, w.squeue2, w.squeue_cl, c->ctr);
-        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(w.squeue2, w.squeue_cl, w.ctl, dout + 8*size_t(off));
+        k_probe_shadow_traversed<<<blocks(m, 256), 256, 0, st>>>(w.squeue2, w.squeue_cl, w.ctl, dout.p + 8*size_t(off));
         if (sc.n_nodes)
             c->ks.shadow_bvh<<<std::min(blocks(m, kTraceBlock), c->persist_blocks), kTraceBlock, 0, st>>>(sc, w.sr, w.squeue2, w.squeue_cl, w.ctl, c->ctr);
-        k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(w.sr, dl + 2*size_t(off), dout + 8*size_t(off), m);
+        k_probe_shadow_read<<<blocks(m, 128), 128, 0, st>>>(w.sr, dl.p + 2*size_t(off), dout.p + 8*size_t(off), m);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = b.download(out, dout, 8*size_t(n));
+    if (e == cudaSuccess) e = download(c, out, dout.p, 8*size_t(n));
     return b.finish(e, "shadow_probe");
 }
 
@@ -1575,15 +1526,15 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
     Wavefront &w = c->wf[0];
     if (int rc = ensure_results(c, w.capacity)) return rc;
     ProbeBufs b(c);
-    uint32_t *din = nullptr, *dout = nullptr, *pix = nullptr;
-    cudaError_t e = b.upload(&din, state_in, TGB_BOUNCE_WORDS*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&dout, TGB_BOUNCE_WORDS*size_t(n));
-    if (e == cudaSuccess) e = b.alloc(&pix, 4*size_t(w.capacity) + 1);
+    Buffer<uint32_t> din, dout, pix;
+    cudaError_t e = din.upload(state_in, TGB_BOUNCE_WORDS*size_t(n), c->stream);
+    if (e == cudaSuccess) e = dout.ensure(TGB_BOUNCE_WORDS*size_t(n));
+    if (e == cudaSuccess) e = pix.ensure(4*size_t(w.capacity) + 1);
     if (e == cudaSuccess) e = b.save_state();
     const DScene &sc = c->sc; cudaStream_t st = c->stream;
     PathBuf &pb = w.pb[0], &dst = w.pb[1];
     // per chunk: one pixel per path (pix_id, pix_seed, pix_first (m + 1 offsets), pix_base), so path id = result slot = its index
-    uint32_t *pix_id = pix, *pix_seed = pix + w.capacity, *pix_base = pix + 2*size_t(w.capacity), *pix_first = pix + 3*size_t(w.capacity);
+    uint32_t *pix_id = pix.p, *pix_seed = pix.p + w.capacity, *pix_base = pix.p + 2*size_t(w.capacity), *pix_first = pix.p + 3*size_t(w.capacity);
     for (uint32_t off = 0; off < n && e == cudaSuccess; off += w.capacity) {
         const uint32_t m = std::min(w.capacity, n - off);
         // the states enter as m survivors k_accum has just handed over, with no camera path left to issue: k_iter_end and
@@ -1596,19 +1547,19 @@ int tgb200_bounce_probe(tgb_ctx *c, uint32_t n, const uint32_t *state_in, uint32
         BatchInfo bi; bi.pix_id = pix_id; bi.pix_seed = pix_seed; bi.n_pix = m; bi.spp_begin = 0;
         bi.pix_first = pix_first; bi.pix_base = pix_base;
         bi.pix_bits = index_bits(m);
-        uint32_t *o = dout + TGB_BOUNCE_WORDS*size_t(off);
-        k_probe_bounce_setup<<<blocks(m, 256), 256, 0, st>>>(sc, pb, din + TGB_BOUNCE_WORDS*size_t(off), pix_id, pix_seed, pix_first,
+        uint32_t *o = dout.p + TGB_BOUNCE_WORDS*size_t(off);
+        k_probe_bounce_setup<<<blocks(m, 256), 256, 0, st>>>(sc, pb, din.p + TGB_BOUNCE_WORDS*size_t(off), pix_id, pix_seed, pix_first,
                                                             pix_base, w.bin_keys, w.bin_hist, o, m);
         k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, sc.n_nodes ? 1 : 0);
         if (sc.n_nodes) k_bin_scatter<<<loop_grid(c->scatter_blocks, m), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
         enqueue_bounce(c, w, pb, dst, st, bi, m, nullptr);
         k_probe_bounce_alive<<<blocks(m, 256), 256, 0, st>>>(dst, w.ctl, o);
-        k_probe_bounce_finished<<<blocks(m, 256), 256, 0, st>>>(pb, c->R, o, m);
+        k_probe_bounce_finished<<<blocks(m, 256), 256, 0, st>>>(pb, c->R.p, o, m);
         e = cudaGetLastError();
         // (the next chunk's control block is copied from this host variable: wait until this one is consumed)
         if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     }
-    if (e == cudaSuccess) e = b.download(state_out, dout, TGB_BOUNCE_WORDS*size_t(n));
+    if (e == cudaSuccess) e = download(c, state_out, dout.p, TGB_BOUNCE_WORDS*size_t(n));
     return b.finish(e, "bounce_probe");
 }
 
@@ -1620,8 +1571,8 @@ int tgb200_bin_probe(tgb_ctx *c, uint32_t n, const uint32_t *keys, uint32_t *ord
         if (keys[i] > kBins) return fail(c, TGB_ERR_INVALID, "survivor %u: key %u is past kBins (%u)", i, keys[i], kBins);
     CU(cudaSetDevice(c->device));
     ProbeBufs b(c);
-    uint32_t *dkeys = nullptr;
-    cudaError_t e = b.upload(&dkeys, keys, n);
+    Buffer<uint32_t> dkeys;
+    cudaError_t e = dkeys.upload(keys, n, c->stream);
     if (e == cudaSuccess) e = b.save_state();
     const cudaStream_t st = c->stream;
     // n survivors just handed over by k_accum, with no camera path left to issue (as tgb200_bounce_probe stages them)
@@ -1630,16 +1581,16 @@ int tgb200_bin_probe(tgb_ctx *c, uint32_t n, const uint32_t *keys, uint32_t *ord
     if (e == cudaSuccess) e = cudaMemcpyAsync(w.ctl, &init, sizeof(Ctl), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemsetAsync(w.bin_hist, 0, kBins*sizeof(uint32_t), st);
     if (e == cudaSuccess) {
-        k_probe_bin_setup<<<blocks(n, 256), 256, 0, st>>>(dkeys, w.bin_keys, w.bin_hist, n);
+        k_probe_bin_setup<<<blocks(n, 256), 256, 0, st>>>(dkeys.p, w.bin_keys, w.bin_hist, n);
         k_iter_end<<<1, 1024, 0, st>>>(w.bin_hist, w.ctl, 1);
         k_bin_scatter<<<loop_grid(c->scatter_blocks, n), 256, 0, st>>>(w.bin_keys, w.bin_hist, w.ctl, w.order);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = b.download(n_sorted, &w.ctl->n_sorted, 1);
-    if (e == cudaSuccess) e = b.download(cursors, w.bin_hist, kBins);
+    if (e == cudaSuccess) e = download(c, n_sorted, &w.ctl->n_sorted, 1);
+    if (e == cudaSuccess) e = download(c, cursors, w.bin_hist, kBins);
     // (init and n_sorted are host variables the stream reads and writes: wait before reading n_sorted or leaving)
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e == cudaSuccess && *n_sorted) e = b.download(order, w.order, std::min(*n_sorted, n));
+    if (e == cudaSuccess && *n_sorted) e = download(c, order, w.order, std::min(*n_sorted, n));
     return b.finish(e, "bin_probe");
 }
 
